@@ -1,8 +1,16 @@
-// Experiment harness (not product code): launch-shape / occupancy / control-flow variants of the fused UYVY -> DXT kernels, timed with
-// CUDA events on four rotating 8K frames (264 MB > L2) and compared byte for byte with the shipped kernel's output.
+// Experiment harness (not product code): where the time of the fused UYVY -> DXT1 encode goes, and the launch shapes / loop structures it
+// was chosen from.  Every variant is timed with CUDA events on four rotating 8K frames (265 MB, more than L2) and compared byte for byte
+// with the output of the shipped entry point.
+//   shipped             ugb200_uyvy_to_dxt1_async as the library launches it (dxt_uyvy_kernel<1,2,false>: skew_t64_m12)
+//   oneshot_bB_tT_mM    one thread = B blocks, T-thread CTAs, __launch_bounds__(T, M), one CTA per T B-block strip of a block row
+//   compute_only_*      the one-shot kernel with its input words made from the thread index and a runtime seed (no loads)
+//   memory_only_*       the one-shot loads and store with trivial work in between
+//   skew_tT_mM          one-shot, the two blocks of a thread one phase apart (dxt1_encode_uyvy_pair_skewed)
+//   persist_*           persistent grid (SMs x resident CTAs), static round-robin of 64-block items per warp; pf1 = next item loaded into
+//                       registers before the current one is encoded, pf0 = no look-ahead, l2 = next item prefetched into L2 only
 // Build: nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a --expt-relaxed-constexpr -o tools/exp_dxt tools/exp_dxt.cu
-// Run:   tools/exp_dxt            all variants, one line each
-//        tools/exp_dxt one NAME   that variant only, 3 launches (for ncu)
+// Run:   tools/exp_dxt [rounds, default 60]
+#include <algorithm>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -12,386 +20,132 @@
 
 namespace ugb {
 
-/// experiment: dxt6_encode() with the alpha thresholds computed before the colour indices and both index computations in one loop over pixel
-/// pairs (ALU-only alpha compares between the FMA-heavy colour distances); same operations, same bits
-__device__ __forceinline__ uint4 dxt6_encode_fused(const float (&r)[16], const float (&g)[16], const float (&b)[16])
+enum { ENCODE = 0, COMPUTE_ONLY = 1, MEMORY_ONLY = 2, SKEWED = 3 };
+
+template <int BPT>
+__device__ __forceinline__ void load_words(const uint8_t *p, long step, uint32_t (&w)[4][2 * BPT])
 {
-        const double offd = (double) kOffset;
-        float Y[16];
-        float2 Co[8], Cg[8];  // pixels 2 j (.x) and 2 j + 1 (.y): the pairing of the packed instructions below
-        // ConvertRGBToYCoCg (:141-148): unsuffixed literals make these double expressions, narrowed once.  As compiled:
-        //   Y  = ((r + 2 g) + b) * 0.25,  Co = fma((2 r - 2 b), 0.25, off),  Cg = fma(((-r + 2 g) - b), 0.25, off)
-        // with g2 = g + g.  Written here with fewer FP64 instructions, each step the same real number rounded once: r + g2 = fma(g, 2, r)
-        // (2 g is exact), 2 r - 2 b = 2 (r - b) exactly (scaling by 2 commutes with rounding) and fma(2 d, 0.25, off) = fma(d, 0.5, off).
 #pragma unroll
-        for (int i = 0; i < 16; ++i) {
-                const double dr = (double) r[i], dg = (double) g[i], db = (double) b[i];
-                Y[i] = __double2float_rn(__dmul_rn(__dadd_rn(__fma_rn(dg, 2.0, dr), db), 0.25));
-                const float co = __double2float_rn(__fma_rn(__dadd_rn(dr, -db), 0.5, offd));
-                const float cg = __double2float_rn(__fma_rn(__dadd_rn(__fma_rn(dg, 2.0, -dr), -db), 0.25, offd));
-                if (i & 1) {
-                        Co[i >> 1].y = co, Cg[i >> 1].y = cg;
+        for (int y = 0; y < 4; ++y, p += step) {
+                if (BPT == 1) {
+                        const uint2 v = ld_stream_v2(p);
+                        w[y][0] = v.x, w[y][1] = v.y;
                 } else {
-                        Co[i >> 1].x = co, Cg[i >> 1].x = cg;
+#pragma unroll
+                        for (int q = 0; q < BPT / 2; ++q) {
+                                const uint4 v = ld_stream_v4(p + 16 * q);
+                                w[y][4 * q] = v.x, w[y][4 * q + 1] = v.y, w[y][4 * q + 2] = v.z, w[y][4 * q + 3] = v.w;
+                        }
                 }
         }
-        // FindMinMaxColorsBox (:159-168)
-        float mnY = Y[0], mxY = Y[0], mnCo = Co[0].x, mxCo = Co[0].x, mnCg = Cg[0].x, mxCg = Cg[0].x;
-#pragma unroll
-        for (int i = 1; i < 16; ++i) {
-                mnY = fminf(mnY, Y[i]), mxY = fmaxf(mxY, Y[i]);
-        }
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-                mnCo = fminf(mnCo, fminf(Co[j].x, Co[j].y)), mxCo = fmaxf(mxCo, fmaxf(Co[j].x, Co[j].y));
-                mnCg = fminf(mnCg, fminf(Cg[j].x, Cg[j].y)), mxCg = fmaxf(mxCg, fmaxf(Cg[j].x, Cg[j].y));
-        }
-        // SelectYCoCgDiagonal (:260-270): t = c - (max+min)*0.5 is fma(max+min, -0.5, c); cov sequential from +0
-        {
-                const float sCo = __fadd_rn(mnCo, mxCo), sCg = __fadd_rn(mnCg, mxCg);
-                float cov = 0.0f;
-                const float2 so2 = dup(sCo), sg2 = dup(sCg), mh = dup(-0.5f);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {  // the two deviations of pixels 2 j, 2 j + 1 packed; the chain itself stays sequential
-                        const float2 eo = __ffma2_rn(so2, mh, Co[j]), eg = __ffma2_rn(sg2, mh, Cg[j]);
-                        cov = __fmaf_rn(eo.x, eg.x, cov);
-                        cov = __fmaf_rn(eo.y, eg.y, cov);
-                }
-                if (cov < 0.0f) {  // :485-489
-                        const float t = mxCg;
-                        mxCg = mnCg, mnCg = t;
-                }
-        }
-        // ScaleYCoCg (:241-258)
-        const float eXo = __fadd_rn(mxCo, -kOffset), eXg = __fadd_rn(mxCg, -kOffset);
-        const float eNo = __fadd_rn(mnCo, -kOffset), eNg = __fadd_rn(mnCg, -kOffset);
-        const float m = fmaxf(fmaxf(fabsf(eNo), fabsf(eNg)), fmaxf(fabsf(eXo), fabsf(eXg)));
-        uint32_t scale = 1u;
-        if (m < 0.2509804069995880127f) {  // (float)(64.0/255.0)
-                scale = 2u;
-        }
-        if (m < 0.12549020349979400635f) {  // (float)(32.0/255.0)
-                scale = 4u;
-        }
-        const float fs = (float) scale, inv_s = scale == 1u ? 1.0f : scale == 2u ? 0.5f : 0.25f;  // rcp.rn of 1,2,4 is exact
-
-        // EmitEndPointsYCoCgDXT5 (:272-313)
-        const float sXo = __fmaf_rn(eXo, fs, kOffset), sXg = __fmaf_rn(eXg, fs, kOffset);  // (c - off)*scale + off
-        const float sNo = __fmaf_rn(eNo, fs, kOffset), sNg = __fmaf_rn(eNg, fs, kOffset);
-        // InsetCoCgBBox (:182-187): (max-min)*(1/16) - (float)((8/255)/16) in one FMA
-        const float kIns = (float) ((8.0 / 255.0) / 16.0);  // 0.0019607844...
-        const float insO = __fmaf_rn(__fadd_rn(sXo, -sNo), 0.0625f, -kIns), insG = __fmaf_rn(__fadd_rn(sXg, -sNg), 0.0625f, -kIns);
-        const float cXo = add_sat_rn(sXo, -insO), cXg = add_sat_rn(sXg, -insG);  // clamp(max - inset, 0, 1)
-        const float cNo = add_sat_rn(sNo, insO), cNg = add_sat_rn(sNg, insG);    // clamp(min + inset, 0, 1)
-        const uint32_t qXo = magic_bits(roundu_magic(__fmul_rn(cXo, 31.0f))), qXg = magic_bits(roundu_magic(__fmul_rn(cXg, 63.0f)));
-        const uint32_t qNo = magic_bits(roundu_magic(__fmul_rn(cNo, 31.0f))), qNg = magic_bits(roundu_magic(__fmul_rn(cNg, 63.0f)));
-        uint4 outp;
-        outp.z = ((qXo << 11) | (qXg << 5) | (scale - 1u)) | (((qNo << 11) | (qNg << 5) | (scale - 1u)) << 16);
-        // expand to 8 bits, back to unit range, undo the scale: fma(fma(float(e), 1/255, -off), 1/scale, off)
-        const float k255 = 0.0039215688593685626984f;  // (float)(1.0/255.0)
-#define UGB_EXPAND(q5or6, e)                                                                                           \
-        __fmaf_rn(__fmaf_rn((float) (e), k255, -kOffset), inv_s, kOffset)
-        const float pXo = UGB_EXPAND(qXo, (qXo << 3) | (qXo >> 2)), pXg = UGB_EXPAND(qXg, (qXg << 2) | (qXg >> 4));
-        const float pNo = UGB_EXPAND(qNo, (qNo << 3) | (qNo >> 2)), pNg = UGB_EXPAND(qNg, (qNg << 2) | (qNg >> 4));
-#undef UGB_EXPAND
-
-        // EmitIndicesYCoCgDXT5 (:315-348).  Palette c0 = max, c1 = min, c2/c3 = lerp with (float)(1/3), (float)(2/3);
-        // which product is the plain multiply and which rides the FMA differs between Co and Cg (as compiled).
-        const float c2o = __fmaf_rn(pNo, 0.3333333432674407959f, __fmul_rn(pXo, 0.66666662693023681641f));
-        const float c2g = __fmaf_rn(pXg, 0.66666662693023681641f, __fmul_rn(pNg, 0.3333333432674407959f));
-        const float c3o = __fmaf_rn(pXo, 0.3333333134651184082f, __fmul_rn(pNo, 0.6666666865348815918f));
-        const float c3g = __fmaf_rn(pXg, 0.3333333134651184082f, __fmul_rn(pNg, 0.6666666865348815918f));
-        // InsetYBBox (:176-181): (max - min)/32.0 - (16.0/255.0)/32.0 in double, narrowed once
-        const float insY = __double2float_rn(__fma_rn((double) __fadd_rn(mxY, -mnY), 1.0 / 32.0, -((16.0 / 255.0) / 32.0)));
-        const float nY = add_sat_rn(mnY, insY), xY = add_sat_rn(mxY, -insY);
-        // EmitAlphaEndPointsYCoCgDXT5 (:350-357): roundf(c * 255.0); the double product narrows to the float product
-        const uint32_t a0 = magic_bits(roundu_magic(__fmul_rn(nY, 255.0f))), a1 = magic_bits(roundu_magic(__fmul_rn(xY, 255.0f)));
-        // EmitAlphaIndicesYCoCgDXT5 (:360-410)
-        const float mid = __fdiv_rn(__fadd_rn(xY, -nY), 14.0f);  // (max-min)/(2.0*7.0): float division is what was compiled
-        const double dX = (double) xY, dN = (double) nY, dM = (double) mid;
-        const double k7 = 1.0 / 7.0;
-        float ab[7];
-        ab[0] = __fadd_rn(nY, mid);
-        ab[1] = __double2float_rn(__fma_rn(__fma_rn(dX, 6.0, dN), k7, dM));
-        ab[2] = __double2float_rn(__fma_rn(__fma_rn(dX, 5.0, __dadd_rn(dN, dN)), k7, dM));
-        ab[3] = __double2float_rn(__fma_rn(__fma_rn(dX, 4.0, __dmul_rn(dN, 3.0)), k7, dM));
-        ab[4] = __double2float_rn(__fma_rn(__fma_rn(dX, 3.0, __dmul_rn(dN, 4.0)), k7, dM));
-        ab[5] = __double2float_rn(__fma_rn(__fma_rn(dX, 2.0, __dmul_rn(dN, 5.0)), k7, dM));
-        ab[6] = __double2float_rn(__fma_rn(__fma_rn(dN, 6.0, dX), k7, dM));
-        // index = 1 + #{k : Y <= ab_k}, & 7, ^ (2 > index)  (:376-388).  The thresholds are ordered ab2 >= ab3 >= ... >= ab7 >= ab1
-        // (rounding is monotone and max >= min), so the count is a 3-step binary search instead of 7 compares, and the
-        // "& 7, ^ (2 > idx)" fix-up is the map 0,2,3,4,5,6,7,1 of the count (alpha_count_to_index).
-        const float T0 = ab[1], T1 = ab[2], T2 = ab[3], T3 = ab[4], T4 = ab[5], T5 = ab[6], T6 = ab[0];
-        uint32_t cntA = 0, cntB = 0;
-        // colorDistance = fma(dCo, dCo, dCg*dCg) for the four palette entries; pixels i and i+1 are computed as a pair —
-        // same operations, half the issue slots
-        uint32_t cidx = 0;
-        const float2 nXo = dup(-pXo), nXg = dup(-pXg), nNo = dup(-pNo), nNg = dup(-pNg), n2o = dup(-c2o), n2g = dup(-c2g), n3o = dup(-c3o),
-                     n3g = dup(-c3g);
-#pragma unroll
-        for (int i = 0; i < 16; i += 2) {
-                const float2 co = Co[i >> 1], cg = Cg[i >> 1];
-#define UGB_DIST2(no, ng, d)                                                                                                               \
-        {                                                                                                                                  \
-                const float2 eo = __fadd2_rn(co, no), eg = __fadd2_rn(cg, ng);                                                             \
-                d = __ffma2_rn(eo, eo, __fmul2_rn(eg, eg));                                                                                \
-        }
-                float2 d0, d1, d2, d3;
-                UGB_DIST2(nXo, nXg, d0)
-                UGB_DIST2(nNo, nNg, d1)
-                UGB_DIST2(n2o, n2g, d2)
-                UGB_DIST2(n3o, n3g, d3)
-#undef UGB_DIST2
-                color_index_bits(cidx, d0.x, d1.x, d2.x, d3.x, 1u << (2 * i), 2u << (2 * i));
-                color_index_bits(cidx, d0.y, d1.y, d2.y, d3.y, 1u << (2 * i + 2), 2u << (2 * i + 2));
-                alpha_count_bits(i < 10 ? cntA : cntB, Y[i], T0, T1, T2, T3, T4, T5, T6, 1u << (3 * (i < 10 ? i : i - 10)));
-                alpha_count_bits(i + 1 < 10 ? cntA : cntB, Y[i + 1], T0, T1, T2, T3, T4, T5, T6, 1u << (3 * (i + 1 < 10 ? i + 1 : i - 9)));
-        }
-        outp.w = cidx;
-
-        const uint32_t idxA = alpha_count_to_index(cntA), idxB = alpha_count_to_index(cntB);
-        // the 48-bit index string (pixel i at bit 3 i) follows the two endpoint bytes (:389-392)
-        const uint32_t s_lo = idxA | (idxB << 30), s_hi = idxB >> 2;
-        outp.x = (a0 << 8) | a1 | (s_lo << 16);
-        outp.y = (s_lo >> 16) | (s_hi << 16);
-        return outp;
 }
 
-
-template <int TPB, int MINB>
-__global__ void __launch_bounds__(TPB, MINB) exp_fused6_kernel(const uint8_t *__restrict__ src, void *__restrict__ out, int wb, int h, long pitch)
+template <int BPT, int MODE>
+__device__ __forceinline__ void encode_store(const uint32_t (&w)[4][2 * BPT], uint2 *o, bool store = true)
 {
-        const int gx = blockIdx.x * blockDim.x + threadIdx.x;
-        const int by = blockIdx.y;
-        if (gx >= wb) {
+        uint2 res[BPT];
+        if (MODE == MEMORY_ONLY) {
+#pragma unroll
+                for (int k = 0; k < BPT; ++k) {
+                        res[k] = make_uint2(w[0][2 * k] ^ w[1][2 * k] ^ w[2][2 * k] ^ w[3][2 * k], w[0][2 * k + 1] ^ w[1][2 * k + 1] ^ w[2][2 * k + 1] ^ w[3][2 * k + 1]);
+                }
+        } else if (MODE == SKEWED) {
+                static_assert(MODE != SKEWED || BPT == 2, "the skewed encode takes two blocks");
+                const uint4 v[4] = { make_uint4(w[0][0], w[0][1], w[0][2], w[0][3]), make_uint4(w[1][0], w[1][1], w[1][2], w[1][3]),
+                                     make_uint4(w[2][0], w[2][1], w[2][2], w[2][3]), make_uint4(w[3][0], w[3][1], w[3][2], w[3][3]) };
+                const uint4 r = dxt1_encode_uyvy_pair_skewed(v);
+                res[0] = make_uint2(r.x, r.y), res[BPT - 1] = make_uint2(r.z, r.w);
+        } else {
+#pragma unroll
+                for (int k = 0; k < BPT; ++k) {
+                        const uint32_t wk[4][2] = { { w[0][2 * k], w[0][2 * k + 1] }, { w[1][2 * k], w[1][2 * k + 1] },
+                                                    { w[2][2 * k], w[2][2 * k + 1] }, { w[3][2 * k], w[3][2 * k + 1] } };
+                        res[k] = dxt1_encode_uyvy_packed(wk);
+                }
+        }
+        if (!store) {
                 return;
         }
-        const uint8_t *p = src + (long) (by * 4) * pitch + gx * 8;
-        float r[16], g[16], b[16];
+        if (BPT == 1) {
+                *o = res[0];
+        } else {
 #pragma unroll
-        for (int y = 0; y < 4; ++y, p += pitch) {
-                const uint2 v = ld_stream_v2(p);
-                load_row_uyvy_packed(v.x, v.y, r + 4 * y, g + 4 * y, b + 4 * y);
+                for (int k = 0; k < BPT; k += 2) {
+                        *(uint4 *) (o + k) = make_uint4(res[k].x, res[k].y, res[k + 1].x, res[k + 1].y);
+                }
         }
-        ((uint4 *) out)[(long) by * wb + gx] = dxt6_encode_fused(r, g, b);
 }
 
-
-template <int DXT_TYPE, int BPT, int TPB, int MINB, bool BRANCH>
-__global__ void __launch_bounds__(TPB, MINB) exp_kernel(const uint8_t *__restrict__ src, void *__restrict__ out, int wb, int h, long pitch)
+/// one-shot grid, as shipped: x over groups of BPT blocks of a block row, y = block row
+template <int BPT, int TPB, int MINB, int MODE>
+__global__ void __launch_bounds__(TPB, MINB) exp_oneshot_kernel(const uint8_t *__restrict__ src, uint2 *__restrict__ out, int wb, int h, long pitch, uint32_t seed)
 {
-        typedef typename block_out<DXT_TYPE>::type out_t;
         const int gx = blockIdx.x * blockDim.x + threadIdx.x;
         const int by = blockIdx.y;
         if (gx >= wb / BPT) {
                 return;
         }
-        const uint8_t *p = src + (long) (by * 4) * pitch + gx * (8 * BPT);
         uint32_t w[4][2 * BPT];
+        if (MODE == COMPUTE_ONLY) {  // words the compiler cannot know: a hash of the position and a runtime seed
+                const uint32_t base = ((uint32_t) by * 0x9E3779B1u + (uint32_t) gx) * 0x85EBCA6Bu ^ seed;
 #pragma unroll
-        for (int y = 0; y < 4; ++y, p += pitch) {
-                if (BPT == 2) {
-                        const uint4 v = ld_stream_v4(p);
-                        w[y][0] = v.x, w[y][1] = v.y, w[y][2] = v.z, w[y][3] = v.w;
-                } else {
-                        const uint2 v = ld_stream_v2(p);
-                        w[y][0] = v.x, w[y][1] = v.y;
-                }
-        }
-        out_t res[BPT];
+                for (int y = 0; y < 4; ++y) {
 #pragma unroll
-        for (int k = 0; k < BPT; ++k) {
-                if constexpr (DXT_TYPE == 1) {
-                        const uint32_t wk[4][2] = { { w[0][2 * k], w[0][2 * k + 1] }, { w[1][2 * k], w[1][2 * k + 1] },
-                                                    { w[2][2 * k], w[2][2 * k + 1] }, { w[3][2 * k], w[3][2 * k + 1] } };
-                        res[k] = dxt1_encode_uyvy_packed<BRANCH>(wk);
-                } else {
-                        float r[16], g[16], b[16];
-#pragma unroll
-                        for (int y = 0; y < 4; ++y) {
-                                load_row_uyvy(w[y][2 * k], w[y][2 * k + 1], r + 4 * y, g + 4 * y, b + 4 * y);
+                        for (int k = 0; k < 2 * BPT; ++k) {
+                                w[y][k] = base * (2u * (8 * y + k) + 1u) + seed;
                         }
-                        res[k] = encode_block<DXT_TYPE>(r, g, b);
                 }
-        }
-        out_t *o = (out_t *) out + ((long) by * wb + gx * BPT);
-        if (DXT_TYPE == 1 && BPT == 2) {
-                *(uint4 *) o = make_uint4(((uint2 *) res)[0].x, ((uint2 *) res)[0].y, ((uint2 *) res)[1].x, ((uint2 *) res)[1].y);
         } else {
-#pragma unroll
-                for (int k = 0; k < BPT; ++k) {
-                        o[k] = res[k];
-                }
+                load_words<BPT>(src + (long) (by * 4) * pitch + (long) gx * (8 * BPT), pitch, w);
         }
+        encode_store<BPT, MODE>(w, out + ((long) by * wb + (long) gx * BPT));
 }
 
-
-__device__ __forceinline__ void spin_cycles(long long n)
+/// persistent grid, two blocks per thread: warp g of W takes the items (32 pairs of one block row) g, g + W, ...; the look-ahead (PF) and the
+/// encode (MODE) are knobs
+template <int TPB, int MINB, int MODE, int PF>
+__global__ void __launch_bounds__(TPB, MINB) exp_persist_kernel(const uint8_t *__restrict__ src, uint2 *__restrict__ out, int wb, int h, long pitch, uint32_t)
 {
-        const long long t0 = clock64();
-        while (clock64() - t0 < n) {
+        const int pairs = wb / 2, segs = (pairs + 31) / 32, hb = h / 4;
+        const int lane = threadIdx.x & 31;
+        const int warp = blockIdx.x * (TPB / 32) + (threadIdx.x >> 5), nwarps = gridDim.x * (TPB / 32);
+        const int dby = nwarps / segs, dseg = nwarps - dby * segs;
+        int by = warp / segs, seg = warp - by * segs;
+        auto addr = [&](int row, int item) { return src + (long) (4 * row) * pitch + (long) min(item * 32 + lane, pairs - 1) * 16; };
+        uint32_t nxt[4][4];
+        if (PF == 1 && by < hb) {
+                load_words<2>(addr(by, seg), pitch, nxt);
         }
-}
-
-/// one-shot kernel with a start skew: the CTAs of the first wave wait a pseudo-random time in [0, SKEW) cycles -
-/// the CTAs that follow inherit the offsets, so that the warps of an SM are spread over the phases of the block encode instead of marching
-/// through them together (conversion = FMA + ALU, bounding box = ALU only, covariance / projection = FMA only)
-template <int DXT_TYPE, int BPT, int TPB, int MINB, int SKEW>
-__global__ void __launch_bounds__(TPB, MINB) exp_skew_kernel(const uint8_t *__restrict__ src, void *__restrict__ out, int wb, int h, long pitch)
-{
-        typedef typename block_out<DXT_TYPE>::type out_t;
-        const int lin = blockIdx.y * gridDim.x + blockIdx.x;
-        if (lin < 148 * MINB) {
-                spin_cycles((long long) (((lin * 2654435761u) >> 16) * (unsigned) SKEW >> 16));  // uniform in [0, SKEW)
-        }
-        const int gx = blockIdx.x * blockDim.x + threadIdx.x;
-        const int by = blockIdx.y;
-        if (gx >= wb / BPT) {
-                return;
-        }
-        const uint8_t *p = src + (long) (by * 4) * pitch + gx * (8 * BPT);
-        uint32_t w[4][2 * BPT];
-#pragma unroll
-        for (int y = 0; y < 4; ++y, p += pitch) {
-                if (BPT == 2) {
-                        const uint4 v = ld_stream_v4(p);
-                        w[y][0] = v.x, w[y][1] = v.y, w[y][2] = v.z, w[y][3] = v.w;
-                } else {
-                        const uint2 v = ld_stream_v2(p);
-                        w[y][0] = v.x, w[y][1] = v.y;
-                }
-        }
-        out_t res[BPT];
-#pragma unroll
-        for (int k = 0; k < BPT; ++k) {
-                if constexpr (DXT_TYPE == 1) {
-                        const uint32_t wk[4][2] = { { w[0][2 * k], w[0][2 * k + 1] }, { w[1][2 * k], w[1][2 * k + 1] },
-                                                    { w[2][2 * k], w[2][2 * k + 1] }, { w[3][2 * k], w[3][2 * k + 1] } };
-                        res[k] = dxt1_encode_uyvy_packed<true>(wk);
-                } else {
-                        float r[16], g[16], b[16];
-#pragma unroll
-                        for (int y = 0; y < 4; ++y) {
-                                load_row_uyvy(w[y][2 * k], w[y][2 * k + 1], r + 4 * y, g + 4 * y, b + 4 * y);
-                        }
-                        res[k] = encode_block<DXT_TYPE>(r, g, b);
-                }
-        }
-        out_t *o = (out_t *) out + ((long) by * wb + gx * BPT);
-        if (DXT_TYPE == 1 && BPT == 2) {
-                *(uint4 *) o = make_uint4(((uint2 *) res)[0].x, ((uint2 *) res)[0].y, ((uint2 *) res)[1].x, ((uint2 *) res)[1].y);
-        } else {
-#pragma unroll
-                for (int k = 0; k < BPT; ++k) {
-                        o[k] = res[k];
-                }
-        }
-}
-
-/// persistent kernel: 148 * MINB CTAs; a warp takes items (32 * BPT horizontally adjacent blocks of one block row) round-robin
-/// (DYN = false) or from an atomic counter (DYN = true), and fetches the next item's rows into registers before it encodes the current one.
-/// SKEW: every warp starts after a pseudo-random delay in [0, SKEW) cycles.
-template <int DXT_TYPE, int BPT, int TPB, int MINB, bool DYN, int SKEW, int PF = 1>
-__global__ void __launch_bounds__(TPB, MINB) exp_persist_kernel(const uint8_t *__restrict__ src, void *__restrict__ out, int wb, int h, long pitch,
-                                                                 unsigned *__restrict__ counter)
-{
-        typedef typename block_out<DXT_TYPE>::type out_t;
-        constexpr int WPC = TPB / 32;
-        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        const int groups_per_row = (wb / BPT + 31) / 32;
-        const int nitems = groups_per_row * (h / 4);
-        const int total_warps = gridDim.x * WPC;
-        if (SKEW > 0) {  // uniform in [0, SKEW)
-                spin_cycles((long long) ((((blockIdx.x * WPC + warp) * 2654435761u) >> 16) * (unsigned) SKEW >> 16));
-        }
-        auto next_item = [&](int cur) -> int {
-                if (DYN) {
-                        unsigned v = 0;
-                        if (lane == 0) {
-                                v = atomicAdd(counter, 1u);
-                        }
-                        return (int) __shfl_sync(0xffffffffu, v, 0);
-                }
-                return cur < 0 ? blockIdx.x * WPC + warp : cur + total_warps;
-        };
-        auto load_item = [&](int item, uint32_t (&w)[4][2 * BPT]) {
-                const int by = item / groups_per_row, gx = (item - by * groups_per_row) * 32 + lane;
-                const bool ok = gx < wb / BPT;
-                const uint8_t *p = src + (long) (by * 4) * pitch + (ok ? gx : 0) * (8 * BPT);
-#pragma unroll
-                for (int y = 0; y < 4; ++y, p += pitch) {
-                        if (BPT == 2) {
-                                const uint4 v = ld_stream_v4(p);
-                                w[y][0] = v.x, w[y][1] = v.y, w[y][2] = v.z, w[y][3] = v.w;
-                        } else {
-                                const uint2 v = ld_stream_v2(p);
-                                w[y][0] = v.x, w[y][1] = v.y;
-                        }
-                }
-        };
-        auto prefetch_item = [&](int item) {  // PF == 2: pull the next item's rows into L2 while this one is encoded (no registers held)
-                const int by = item / groups_per_row, gx = (item - by * groups_per_row) * 32 + lane;
-                const uint8_t *p = src + (long) (by * 4) * pitch + (gx < wb / BPT ? gx : 0) * (8 * BPT);
-#pragma unroll
-                for (int y = 0; y < 4; ++y, p += pitch) {
-                        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-                }
-        };
-        int item = next_item(-1);
-        uint32_t wn[4][2 * BPT];
-        if (PF == 1 && item < nitems) {
-                load_item(item, wn);
-        }
-        while (item < nitems) {
-                uint32_t w[4][2 * BPT];
+        while (by < hb) {
+                uint32_t w[4][4];
                 if (PF == 1) {
 #pragma unroll
                         for (int y = 0; y < 4; ++y) {
 #pragma unroll
-                                for (int k = 0; k < 2 * BPT; ++k) {
-                                        w[y][k] = wn[y][k];
+                                for (int k = 0; k < 4; ++k) {
+                                        w[y][k] = nxt[y][k];
                                 }
                         }
                 } else {
-                        load_item(item, w);
+                        load_words<2>(addr(by, seg), pitch, w);
                 }
-                const int nxt = next_item(item);
-                if (nxt < nitems) {
+                const int gx = seg * 32 + lane, cur = by;
+                seg += dseg, by += dby;
+                if (seg >= segs) {
+                        seg -= segs, ++by;
+                }
+                if (by < hb) {
                         if (PF == 1) {
-                                load_item(nxt, wn);
+                                load_words<2>(addr(by, seg), pitch, nxt);
                         } else if (PF == 2) {
-                                prefetch_item(nxt);
-                        }
-                }
-                out_t res[BPT];
+                                const uint8_t *p = addr(by, seg);
 #pragma unroll
-                for (int k = 0; k < BPT; ++k) {
-                        if constexpr (DXT_TYPE == 1) {
-                                const uint32_t wk[4][2] = { { w[0][2 * k], w[0][2 * k + 1] }, { w[1][2 * k], w[1][2 * k + 1] },
-                                                            { w[2][2 * k], w[2][2 * k + 1] }, { w[3][2 * k], w[3][2 * k + 1] } };
-                                res[k] = dxt1_encode_uyvy_packed<true>(wk);
-                        } else {
-                                float r[16], g[16], b[16];
-#pragma unroll
-                                for (int y = 0; y < 4; ++y) {
-                                        load_row_uyvy(w[y][2 * k], w[y][2 * k + 1], r + 4 * y, g + 4 * y, b + 4 * y);
-                                }
-                                res[k] = encode_block<DXT_TYPE>(r, g, b);
-                        }
-                }
-                const int by = item / groups_per_row, gx = (item - by * groups_per_row) * 32 + lane;
-                if (gx < wb / BPT) {
-                        out_t *o = (out_t *) out + ((long) by * wb + gx * BPT);
-                        if (DXT_TYPE == 1 && BPT == 2) {
-                                *(uint4 *) o = make_uint4(((uint2 *) res)[0].x, ((uint2 *) res)[0].y, ((uint2 *) res)[1].x, ((uint2 *) res)[1].y);
-                        } else {
-#pragma unroll
-                                for (int k = 0; k < BPT; ++k) {
-                                        o[k] = res[k];
+                                for (int y = 0; y < 4; ++y, p += pitch) {
+                                        asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
                                 }
                         }
                 }
-                item = nxt;
+                encode_store<2, MODE>(w, out + ((long) cur * wb + 2 * gx), gx < pairs);
         }
 }
 
@@ -419,117 +173,119 @@ __global__ void fill_kernel(uint32_t *p, long nwords, uint32_t seed, int w_words
 
 }  // namespace ugb
 
+typedef void (*kern_t)(const uint8_t *, uint2 *, int, int, long, uint32_t);
 struct variant {
         std::string name;
-        int dxt, bpt, tpb, minb;  // minb > 0: persistent kernel with 148 * minb CTAs
-        void (*kern)(const uint8_t *, void *, int, int, long);
-        void (*pkern)(const uint8_t *, void *, int, int, long, unsigned *);
+        int bpt, tpb;
+        bool persistent;  // grid = SMs x resident CTAs
+        int mode;
+        kern_t kern;      // nullptr: the shipped entry point
+        std::vector<float> us;
 };
 
-#define KF(T, M) { "d1_fine_t" #T "_m" #M, 1, 2, T, 0, ugb::dxt1_uyvy_skew_kernel<false, T, M, 1>, nullptr }
-#define KR(T, M) { "d1_regions_t" #T "_m" #M, 1, 2, T, 0, ugb::dxt1_uyvy_skew_kernel<false, T, M, 2>, nullptr }
-#define K(T, M) { "d1_skew_t" #T "_m" #M, 1, 2, T, 0, ugb::dxt1_uyvy_skew_kernel<false, T, M>, nullptr }
-#define V(D, B, T, M, BR) { "d" #D "_b" #B "_t" #T "_m" #M "_" #BR, D, B, T, 0, ugb::exp_kernel<D, B, T, M, BR>, nullptr }
-#define S(D, B, T, M, SK) { "d" #D "_b" #B "_t" #T "_m" #M "_skew" #SK, D, B, T, 0, ugb::exp_skew_kernel<D, B, T, M, SK>, nullptr }
-#define F6(T, M) { "d6_fusedloops_t" #T "_m" #M, 6, 1, T, 0, ugb::exp_fused6_kernel<T, M>, nullptr }
-#define P(D, B, T, M, DYN, SK) { "d" #D "_b" #B "_t" #T "_m" #M "_persist_" #DYN "_skew" #SK, D, B, T, M, nullptr, ugb::exp_persist_kernel<D, B, T, M, DYN, SK> }
-#define Q(D, B, T, M, DYN, SK, PF) { "d" #D "_b" #B "_t" #T "_m" #M "_persist_" #DYN "_skew" #SK "_pf" #PF, D, B, T, M, nullptr, ugb::exp_persist_kernel<D, B, T, M, DYN, SK, PF> }
+#define O(B, T, M) { "oneshot_b" #B "_t" #T "_m" #M, B, T, false, ugb::ENCODE, ugb::exp_oneshot_kernel<B, T, M, ugb::ENCODE>, {} }
+#define C(B, T, M) { "compute_only_b" #B "_t" #T "_m" #M, B, T, false, ugb::COMPUTE_ONLY, ugb::exp_oneshot_kernel<B, T, M, ugb::COMPUTE_ONLY>, {} }
+#define MO(B, T, M) { "memory_only_b" #B "_t" #T "_m" #M, B, T, false, ugb::MEMORY_ONLY, ugb::exp_oneshot_kernel<B, T, M, ugb::MEMORY_ONLY>, {} }
+#define K(T, M) { "skew_t" #T "_m" #M, 2, T, false, ugb::SKEWED, ugb::exp_oneshot_kernel<2, T, M, ugb::SKEWED>, {} }
+#define P(T, M, PF) { "persist_t" #T "_m" #M "_pf" #PF, 2, T, true, ugb::ENCODE, ugb::exp_persist_kernel<T, M, ugb::ENCODE, PF>, {} }
+#define PK(T, M) { "persist_skew_t" #T "_m" #M "_pf1", 2, T, true, ugb::SKEWED, ugb::exp_persist_kernel<T, M, ugb::SKEWED, 1>, {} }
+#define PM(T, M) { "persist_memory_only_t" #T "_m" #M, 2, T, true, ugb::MEMORY_ONLY, ugb::exp_persist_kernel<T, M, ugb::MEMORY_ONLY, 1>, {} }
 
 int main(int argc, char **argv)
 {
-        const int W = 7680, H = 4320;
+        const int W = 7680, H = 4320, rounds = argc > 1 ? atoi(argv[1]) : 60;
         const long frame = (long) W * H * 2;
         std::vector<variant> vs = {
-                // DXT1: shipped shape first (two blocks per thread, 64-thread CTAs), then the alternatives that were measured
-                V(1, 2, 64, 12, true), K(64, 8), K(64, 10), K(64, 12), K(64, 6), K(128, 4), K(128, 5), K(32, 16), K(32, 20), KF(64, 8), KF(64, 10), KF(64, 6), KF(128, 4), KF(32, 16), KR(64, 8), KR(64, 10), KR(64, 6), KR(128, 4), KR(32, 16), KR(64, 12), V(1, 2, 128, 6, true), V(1, 2, 32, 24, true), V(1, 2, 256, 3, true), V(1, 2, 64, 12, false), V(1, 2, 64, 10, true),
-                V(1, 1, 64, 14, true), V(1, 1, 128, 8, true), S(1, 2, 64, 12, 2000), S(1, 2, 64, 12, 8000),
-                P(1, 2, 128, 5, false, 1400), P(1, 2, 128, 5, true, 0), Q(1, 2, 128, 6, true, 1400, 2), Q(1, 2, 128, 6, true, 1400, 0),
-                // DXT5-YCoCg
-                V(6, 1, 128, 7, true), F6(128, 7), F6(128, 6), F6(128, 5), V(6, 1, 128, 6, true), V(6, 1, 64, 12, true), V(6, 1, 128, 5, true), V(6, 1, 128, 4, true), V(6, 1, 128, 7, true), V(6, 1, 256, 3, true),
-                S(6, 1, 64, 12, 4000), P(6, 1, 128, 4, true, 1800), Q(6, 1, 128, 6, true, 1800, 2),
+                { "shipped", 2, 0, false, ugb::ENCODE, nullptr, {} },
+                C(2, 64, 12), MO(2, 64, 12), PM(128, 4),
+                O(2, 64, 12), O(2, 64, 10), O(2, 128, 5), O(2, 128, 4), O(1, 64, 12), O(4, 64, 8),
+                K(64, 12), K(64, 10), K(128, 5), K(128, 4),
+                P(128, 4, 1), P(256, 2, 1), P(128, 5, 2), PK(128, 4),
         };
-        const char *only = argc > 2 && !strcmp(argv[1], "one") ? argv[2] : nullptr;
+        int dev = 0, sms = 0;
+        cudaGetDevice(&dev);
+        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        cudaDeviceProp prop;
+        cudaGetDeviceProperties(&prop, dev);
+        printf("device %s, %d SMs\n", prop.name, sms);
 
-        uint8_t *src[4], *out, *ref[2];
-        unsigned *counters;
+        uint8_t *src[4];
+        uint2 *out, *ref;
         for (int i = 0; i < 4; ++i) {
                 cudaMalloc(&src[i], frame + 256);
-                ugb::fill_kernel<<<148 * 8, 256>>>((uint32_t *) src[i], frame / 4, (uint32_t) (i + 1), W * 2 / 4, H);
+                ugb::fill_kernel<<<sms * 8, 256>>>((uint32_t *) src[i], frame / 4, (uint32_t) (i + 1), W * 2 / 4, H);
         }
-        cudaMalloc(&out, (size_t) W * H);
-        cudaMalloc(&ref[0], (size_t) W * H);
-        cudaMalloc(&ref[1], (size_t) W * H);
-        cudaMalloc(&counters, 4096 * sizeof(unsigned));
-        std::vector<uint8_t> h_ref[2], h_out((size_t) W * H);
-        // reference outputs of frame 0 from the shipped entry points
-        ugb200_uyvy_to_dxt1_async(src[0], ref[0], W, H, 0, nullptr);
-        ugb200_uyvy_to_dxt6_async(src[0], ref[1], W, H, 0, nullptr);
+        const size_t out_bytes = (size_t) W * H / 2;
+        cudaMalloc(&out, out_bytes);
+        cudaMalloc(&ref, out_bytes);
+        std::vector<uint8_t> h_ref(out_bytes), h_out(out_bytes);
+        ugb200_uyvy_to_dxt1_async(src[0], ref, W, H, 0, nullptr);
         if (cudaDeviceSynchronize() != cudaSuccess) {
                 printf("setup failed: %s\n", cudaGetErrorString(cudaGetLastError()));
                 return 1;
         }
-        for (int k = 0; k < 2; ++k) {
-                h_ref[k].resize((size_t) W * H / (k == 0 ? 2 : 1));
-                cudaMemcpy(h_ref[k].data(), ref[k], h_ref[k].size(), cudaMemcpyDeviceToHost);
-        }
+        cudaMemcpy(h_ref.data(), ref, out_bytes, cudaMemcpyDeviceToHost);
+        auto launch = [&](const variant &v, dim3 grid, int i) {
+                if (!v.kern) {
+                        ugb200_uyvy_to_dxt1_async(src[i & 3], out, W, H, 0, nullptr);
+                } else {
+                        v.kern<<<grid, v.tpb>>>(src[i & 3], out, W / 4, H, (long) W * 2, 0x9E3779B9u * (i + 1));
+                }
+        };
         cudaEvent_t e0, e1;
         cudaEventCreate(&e0), cudaEventCreate(&e1);
         const int wb = W / 4, hb = H / 4;
-        for (const variant &v : vs) {
-                if (only && v.name != only) {
-                        continue;
+        std::vector<dim3> grids;
+        for (variant &v : vs) {  // attributes, grid, bit-exactness, warm-up
+                int occ = 0, regs = 0;
+                size_t spill = 0;
+                if (v.kern) {
+                        cudaFuncAttributes fa;
+                        cudaFuncGetAttributes(&fa, (const void *) v.kern);
+                        regs = fa.numRegs, spill = fa.localSizeBytes;
+                        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, (const void *) v.kern, v.tpb, 0);
                 }
-                const int groups = wb / v.bpt;
-                const dim3 grid((groups + v.tpb - 1) / v.tpb, hb);
-                const void *fn = v.kern ? (const void *) v.kern : (const void *) v.pkern;
-                int launch_no = 0;
-                auto launch = [&](const uint8_t *s) {
-                        if (v.kern) {
-                                v.kern<<<grid, v.tpb>>>(s, out, wb, H, (long) W * 2);
-                        } else {
-                                v.pkern<<<148 * v.minb, v.tpb>>>(s, out, wb, H, (long) W * 2, counters + (launch_no++ & 4095));
-                        }
-                };
-                cudaFuncAttributes fa;
-                cudaFuncGetAttributes(&fa, fn);
-                int occ = 0;
-                cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, v.tpb, 0);
-                cudaMemset(counters, 0, 4096 * sizeof(unsigned));
-                if (only) {
-                        for (int i = 0; i < 3; ++i) {
-                                launch(src[i]);
-                        }
-                        cudaDeviceSynchronize();
-                        printf("%s ran\n", v.name.c_str());
-                        continue;
-                }
-                const size_t out_bytes = (size_t) W * H / (v.dxt == 1 ? 2 : 1);
+                grids.push_back(v.persistent ? dim3(sms * occ) : dim3((wb / v.bpt + v.tpb - 1) / std::max(v.tpb, 1), hb));
                 cudaMemset(out, 0xEE, out_bytes);
-                launch(src[0]);
+                launch(v, grids.back(), 0);
                 cudaMemcpy(h_out.data(), out, out_bytes, cudaMemcpyDeviceToHost);
-                const bool same = memcmp(h_out.data(), h_ref[v.dxt == 1 ? 0 : 1].data(), out_bytes) == 0;
-                float best = 1e9f, sum = 0;
-                const int reps = 3, iters = v.dxt == 1 ? 40 : 20;
-                for (int r = 0; r < reps; ++r) {
-                        cudaMemset(counters, 0, 4096 * sizeof(unsigned));
-                        launch_no = 0;
-                        cudaDeviceSynchronize();
+                const char *check = v.mode == ugb::ENCODE || v.mode == ugb::SKEWED ? (memcmp(h_out.data(), h_ref.data(), out_bytes) ? "MISMATCH" : "bit-exact") : "-";
+                const cudaError_t err = cudaGetLastError();
+                printf("%-30s regs %3d spill %3zu B  CTAs/SM %2d  warps/SM %2d  %s %s\n", v.name.c_str(), regs, spill, occ, occ * v.tpb / 32, check,
+                       err == cudaSuccess ? "" : cudaGetErrorString(err));
+        }
+        // The card is power-capped, so its SM clock wanders by tens of percent over seconds.  Variants are therefore timed in short windows
+        // (`iters` launches, a few ms), one window per variant per round with the starting variant rotated, over many rounds: every variant
+        // sees the same spread of clocks, and the median over rounds compares them.
+        const int nv = (int) vs.size(), iters = 40;
+        for (int round = 0; round < rounds; ++round) {
+                for (int k = 0; k < nv; ++k) {
+                        const int i = (k + round) % nv;
+                        launch(vs[i], grids[i], round);
                         cudaEventRecord(e0);
-                        for (int i = 0; i < iters; ++i) {
-                                launch(src[i & 3]);
+                        for (int it = 0; it < iters; ++it) {
+                                launch(vs[i], grids[i], it);
                         }
                         cudaEventRecord(e1);
                         cudaEventSynchronize(e1);
                         float ms;
                         cudaEventElapsedTime(&ms, e0, e1);
-                        best = ms < best ? ms : best;
-                        sum += ms;
+                        vs[i].us.push_back(ms / iters * 1e3f);
                 }
-                const cudaError_t err = cudaGetLastError();
-                printf("%-36s regs %3d spill %3zu B  CTAs/SM %2d warps/SM %2d  best %7.2f us  mean %7.2f us  %s%s\n", v.name.c_str(), fa.numRegs,
-                       (size_t) fa.localSizeBytes, occ, occ * v.tpb / 32, best / iters * 1e3, sum / reps / iters * 1e3, same ? "bit-exact" : "MISMATCH",
-                       err == cudaSuccess ? "" : cudaGetErrorString(err));
-                fflush(stdout);
+        }
+        if (cudaGetLastError() != cudaSuccess) {
+                printf("timing failed\n");
+                return 1;
+        }
+        printf("\nus per 8K frame over %d rounds of %d-launch windows: median [quartiles]  (median / median of shipped)\n", rounds, iters);
+        float ship = 0;
+        for (variant &v : vs) {
+                std::sort(v.us.begin(), v.us.end());
+                const size_t n = v.us.size();
+                if (!v.kern) {
+                        ship = v.us[n / 2];
+                }
+                printf("%-30s %7.2f  [%7.2f %7.2f]  %.3f\n", v.name.c_str(), v.us[n / 2], v.us[n / 4], v.us[3 * n / 4], v.us[n / 2] / ship);
         }
         return 0;
 }

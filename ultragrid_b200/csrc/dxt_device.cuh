@@ -233,10 +233,12 @@ __device__ __forceinline__ float px(const float2 (&v)[8], int i) { return ((i & 
 template <bool BRANCH = true>
 __device__ __forceinline__ uint2 dxt1_encode_packed_core(const float2 (&R)[8], const float2 (&G)[8], const float2 (&B)[8])
 {
-        // bounding box
-        float mnr = R[0].x, mng = G[0].x, mnb = B[0].x, mxr = mnr, mxg = mng, mxb = mnb;
+        // bounding box, seeded with the first pixel pair (15 FMNMX per chain)
+        float mnr = fminf(R[0].x, R[0].y), mxr = fmaxf(R[0].x, R[0].y);
+        float mng = fminf(G[0].x, G[0].y), mxg = fmaxf(G[0].x, G[0].y);
+        float mnb = fminf(B[0].x, B[0].y), mxb = fmaxf(B[0].x, B[0].y);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        for (int j = 1; j < 8; ++j) {
                 mnr = fminf(mnr, fminf(R[j].x, R[j].y)), mxr = fmaxf(mxr, fmaxf(R[j].x, R[j].y));
                 mng = fminf(mng, fminf(G[j].x, G[j].y)), mxg = fmaxf(mxg, fmaxf(G[j].x, G[j].y));
                 mnb = fminf(mnb, fminf(B[j].x, B[j].y)), mxb = fmaxf(mxb, fmaxf(B[j].x, B[j].y));
@@ -402,9 +404,12 @@ __device__ __forceinline__ void d1_rgb_row(dxt1_blk &s, uint32_t w0, uint32_t w1
                 s.B[2 * y + k] = __ffma2_rn(u, dup(2.1124f), yy);
         }
 }
+/// bounding box seeded with the first pixel pair; d1_bbox_step() then takes pairs 1..7
 __device__ __forceinline__ void d1_bbox_init(dxt1_blk &s)
 {
-        s.mnr = s.mxr = s.R[0].x, s.mng = s.mxg = s.G[0].x, s.mnb = s.mxb = s.B[0].x;
+        s.mnr = fminf(s.R[0].x, s.R[0].y), s.mxr = fmaxf(s.R[0].x, s.R[0].y);
+        s.mng = fminf(s.G[0].x, s.G[0].y), s.mxg = fmaxf(s.G[0].x, s.G[0].y);
+        s.mnb = fminf(s.B[0].x, s.B[0].y), s.mxb = fmaxf(s.B[0].x, s.B[0].y);
 }
 __device__ __forceinline__ void d1_bbox_step(dxt1_blk &s, int j)
 {
@@ -482,106 +487,6 @@ __device__ __forceinline__ uint2 d1_pack(const dxt1_blk &s)
         return make_uint2(palette, indices);
 }
 
-// ---- the same phases cut into single statements, so that the source order can alternate FMA-pipe and ALU-pipe work instruction by instruction
-//      (kept by ptxas at -O1; at -O3 its list scheduler clusters the pipes again)
-struct d1_rgb_tmp {
-        float2 u, v, yy;
-};
-#define D1_UV(s, t, w0, w1)                                                                                      \
-        t.u = __ffma2_rn(f2(magic_byte(w0, 0), magic_byte(w1, 0)), dup(kInv255), dup(kBiasC));                    \
-        t.v = __ffma2_rn(f2(magic_byte(w0, 2), magic_byte(w1, 2)), dup(kInv255), dup(kBiasC))
-#define D1_YY(s, t, w0, w1, k) t.yy = __fmul2_rn(__ffma2_rn(f2(magic_byte(w0, 1 + 2 * (k)), magic_byte(w1, 1 + 2 * (k))), dup(kInv255), dup(kBiasY)), dup(1.1643f))
-#define D1_R(s, t, i) s.R[i] = __ffma2_rn(t.v, dup(1.7926f), t.yy)
-#define D1_G(s, t, i) s.G[i] = __ffma2_rn(t.v, dup(-0.5328f), __ffma2_rn(t.u, dup(-0.2132f), t.yy))
-#define D1_B(s, t, i) s.B[i] = __ffma2_rn(t.u, dup(2.1124f), t.yy)
-#define D1_BB(s, C, mn, mx, j) s.mn = fminf(s.mn, fminf(s.C[j].x, s.C[j].y)), s.mx = fmaxf(s.mx, fmaxf(s.C[j].x, s.C[j].y))
-
-/// fine-grained form of dxt1_encode_uyvy_pair_skewed(): same operations per block, statement-level alternation of the two blocks
-/// @param opaque  a value the compiler cannot know (never equal to a small negative number): with D1_REGIONS the statements of one row sit in their
-///                own basic block behind a never-taken branch on it, which is where ptxas' scheduler has to stop
-#define D1_IF(n) if (!REGIONS || opaque != -(long) (n))
-template <bool REGIONS>
-__device__ __forceinline__ uint4 dxt1_encode_uyvy_pair_fine(const uint4 (&v)[4], long opaque)
-{
-        dxt1_blk a, b;
-        d1_rgb_tmp t;
-#pragma unroll
-        for (int y = 0; y < 4; ++y) {
-                d1_rgb_row(a, v[y].x, v[y].y, y);
-        }
-        d1_bbox_init(a);
-#pragma unroll
-        for (int y = 0; y < 4; ++y) D1_IF(3 + y) {  // B: unpack + RGB of row y (14 packed FMA-pipe instructions, 8 PRMT)   A: bounding box of pixel pairs 2y, 2y+1 (12 FMNMX3)
-                D1_UV(b, t, v[y].z, v[y].w);
-                D1_BB(a, R, mnr, mxr, 2 * y);
-                D1_YY(b, t, v[y].z, v[y].w, 0);
-                D1_BB(a, G, mng, mxg, 2 * y);
-                D1_R(b, t, 2 * y);
-                D1_BB(a, B, mnb, mxb, 2 * y);
-                D1_G(b, t, 2 * y);
-                D1_B(b, t, 2 * y);
-                D1_BB(a, R, mnr, mxr, 2 * y + 1);
-                D1_YY(b, t, v[y].z, v[y].w, 1);
-                D1_BB(a, G, mng, mxg, 2 * y + 1);
-                D1_R(b, t, 2 * y + 1);
-                D1_G(b, t, 2 * y + 1);
-                D1_BB(a, B, mnb, mxb, 2 * y + 1);
-                D1_B(b, t, 2 * y + 1);
-        }
-        d1_inset(a);
-        d1_bbox_init(b);
-        const float2 mh = dup(-0.5f);
-#pragma unroll
-        for (int y = 0; y < 4; ++y) D1_IF(11 + y) {  // A: deviations + covariance chains of row y (6 packed + 8 scalar FMA)   B: bounding box
-                const float2 er0 = __ffma2_rn(a.sr2, mh, a.R[2 * y]), eb0 = __ffma2_rn(a.sb2, mh, a.B[2 * y]);
-                D1_BB(b, R, mnr, mxr, 2 * y);
-                const float2 eg0 = __ffma2_rn(a.sg2, mh, a.G[2 * y]);
-                a.covx = __fmaf_rn(er0.x, eb0.x, a.covx);
-                D1_BB(b, G, mng, mxg, 2 * y);
-                const float2 er1 = __ffma2_rn(a.sr2, mh, a.R[2 * y + 1]), eb1 = __ffma2_rn(a.sb2, mh, a.B[2 * y + 1]);
-                a.covy = __fmaf_rn(eg0.x, eb0.x, a.covy);
-                D1_BB(b, B, mnb, mxb, 2 * y);
-                const float2 eg1 = __ffma2_rn(a.sg2, mh, a.G[2 * y + 1]);
-                a.covx = __fmaf_rn(er1.x, eb1.x, a.covx);
-                D1_BB(b, R, mnr, mxr, 2 * y + 1);
-                a.covy = __fmaf_rn(eg1.x, eb1.x, a.covy);
-                a.covx = __fmaf_rn(er0.y, eb0.y, a.covx);
-                D1_BB(b, G, mng, mxg, 2 * y + 1);
-                a.covy = __fmaf_rn(eg0.y, eb0.y, a.covy);
-                a.covx = __fmaf_rn(er1.y, eb1.y, a.covx);
-                D1_BB(b, B, mnb, mxb, 2 * y + 1);
-                a.covy = __fmaf_rn(eg1.y, eb1.y, a.covy);
-        }
-        d1_endpoints(a);
-        d1_inset(b);
-#pragma unroll
-        for (int y = 0; y < 4; ++y) D1_IF(19 + y) {  // A: indices of pixel pairs 2y, 2y+1   B: deviations + covariance of row y
-                d1_index_step(a, 2 * y);
-                d1_cov_row(b, y);
-                d1_index_step(a, 2 * y + 1);
-        }
-        d1_endpoints(b);
-        // A's packing (ALU pipe) goes between B's index steps (FMA pipe)
-        constexpr uint32_t kIdxBias = 0x4B000000u * 0x55555555u;
-        uint32_t ia = a.acc0 + a.acc1 - kIdxBias;
-        d1_index_step(b, 0);
-        ia = a.max_code != a.min_code ? ia : 0u;
-        const bool swa = a.max_code < a.min_code;
-        d1_index_step(b, 1);
-        ia = swa ? ~ia : ia;
-        const uint32_t la = ia & 0x55555555u, ma = ia & 0xaaaaaaaau;
-        d1_index_step(b, 2);
-        ia = ma ^ (2 * la + (ma >> 1));
-        d1_index_step(b, 3);
-        const uint32_t pa = swa ? a.min_code + (a.max_code << 16) : a.max_code + (a.min_code << 16);
-#pragma unroll
-        for (int j = 4; j < 8; ++j) {
-                d1_index_step(b, j);
-        }
-        const uint2 rb = d1_pack(b);
-        return make_uint4(pa, ia, rb.x, rb.y);
-}
-
 /// two horizontally adjacent blocks: v[y] = the 16 bytes (8 pixels) of row y
 __device__ __forceinline__ uint4 dxt1_encode_uyvy_pair_skewed(const uint4 (&v)[4])
 {
@@ -594,7 +499,9 @@ __device__ __forceinline__ uint4 dxt1_encode_uyvy_pair_skewed(const uint4 (&v)[4
 #pragma unroll
         for (int y = 0; y < 4; ++y) {  // B: unpack + RGB (FMA pipe, PRMT)   A: bounding box (ALU pipe)
                 d1_rgb_row(b, v[y].z, v[y].w, y);
-                d1_bbox_step(a, 2 * y);
+                if (y > 0) {
+                        d1_bbox_step(a, 2 * y);
+                }
                 d1_bbox_step(a, 2 * y + 1);
         }
         d1_inset(a);
@@ -602,7 +509,9 @@ __device__ __forceinline__ uint4 dxt1_encode_uyvy_pair_skewed(const uint4 (&v)[4
 #pragma unroll
         for (int y = 0; y < 4; ++y) {  // A: deviations + covariance chains (FMA pipe)   B: bounding box (ALU pipe)
                 d1_cov_row(a, y);
-                d1_bbox_step(b, 2 * y);
+                if (y > 0) {
+                        d1_bbox_step(b, 2 * y);
+                }
                 d1_bbox_step(b, 2 * y + 1);
         }
         d1_endpoints(a);

@@ -7,8 +7,8 @@
 //   DXT5-YCoCg output: one uint4 per block                                   (cuda_dxt.cu:507)
 //
 // Kernels (one thread encodes one 4x4 block; all HBM-streaming, no tensor cores):
-//   dxt1_uyvy_kernel<2>   thread = two horizontally adjacent blocks: 4 x LDG.128, 1 x STG.128
-//   dxt1_uyvy_kernel<1>   fallback for (w/4) odd or 8-byte-only aligned buffers
+//   dxt_uyvy_kernel<1,2>  thread = two horizontally adjacent blocks, encoded one phase apart: 4 x LDG.128, 1 x STG.128
+//   dxt_uyvy_kernel<1,1>  fallback for (w/4) odd or 8-byte-only aligned buffers; dxt_uyvy_kernel<6,1> DXT5-YCoCg
 //   dxt_packed3_kernel    cuda_{rgb,yuv}_to_dxt{1,6}: 3 x LDG.32 per row like the reference, but the grid
 //                         is sized in blocks (the reference launches 16x more threads, cuda_dxt.cu:750-751)
 //   yuv422_to_yuv444_kernel  ABI-compat only; the fused kernels never materialise 4:4:4
@@ -66,8 +66,12 @@ __device__ __forceinline__ uint4 encode_block<6>(const float (&r)[16], const flo
 // ------------------------------------------------------------------------------------------------
 // fused UYVY -> DXT.  One thread = BPT horizontally adjacent blocks.
 // ------------------------------------------------------------------------------------------------
-/// CTA shape, chosen with tools/exp_dxt.cu on 8K frames on an earlier GPU and carried over without re-measuring on the H100.  DXT1: 64-thread
-/// CTAs (a block row of an 8K frame is 960 threads, i.e. 15 CTAs of 64 but 7.5 of 128).  DXT5-YCoCg: 128-thread CTAs, 7 per SM.
+/// CTA shape.  DXT1: 64-thread CTAs, 12 per SM (80 registers, no spill; a block row of an 8K frame is 960 threads, i.e. 15 CTAs of 64 but 7.5
+/// of 128).  Measured with tools/exp_dxt.cu on an H100 80GB HBM3 at a 400 W power limit, 8K frames, median of 100 interleaved rounds: the
+/// two-block kernel with the skewed encode 56.4 us; the same with (64, 10) 56.6, with (128, 5) 58.0; the unskewed encode 58.4 at (64, 12),
+/// 57.4 at (64, 10), 58.9 at (128, 5); one block per thread 61.2; a persistent grid with the next item's rows loaded ahead 62.4 (128 registers
+/// leave 16 warps per SM, and the item loop adds integer instructions to an issue-bound kernel).  DXT5-YCoCg: 128-thread CTAs, 7 per SM,
+/// chosen on an earlier GPU and not re-measured on the H100.
 template <int DXT_TYPE>
 struct uyvy_cta {
         static constexpr int threads = DXT_TYPE == 1 ? 64 : 128, min_ctas = DXT_TYPE == 1 ? 12 : 7;
@@ -99,55 +103,28 @@ __global__ void __launch_bounds__(uyvy_cta<DXT_TYPE>::threads, uyvy_cta<DXT_TYPE
                         w[y][0] = v.x, w[y][1] = v.y;
                 }
         }
-        out_t res[BPT];
-#pragma unroll
-        for (int k = 0; k < BPT; ++k) {
-                if constexpr (DXT_TYPE == 1) {  // paired formulation (same operation tree)
-                        const uint32_t wk[4][2] = { { w[0][2 * k], w[0][2 * k + 1] }, { w[1][2 * k], w[1][2 * k + 1] },
-                                                    { w[2][2 * k], w[2][2 * k + 1] }, { w[3][2 * k], w[3][2 * k + 1] } };
-                        res[k] = dxt1_encode_uyvy_packed(wk);
-                } else {
-                        float r[16], g[16], b[16];
-#pragma unroll
-                        for (int y = 0; y < 4; ++y) {
-                                load_row_uyvy_packed(w[y][2 * k], w[y][2 * k + 1], r + 4 * y, g + 4 * y, b + 4 * y);
-                        }
-                        res[k] = encode_block<DXT_TYPE>(r, g, b);
-                }
-        }
         out_t *o = (out_t *) out + ((long) by * wb + gx * BPT);
-        if (DXT_TYPE == 1 && BPT == 2) {
-                *(uint4 *) o = make_uint4(((uint2 *) res)[0].x, ((uint2 *) res)[0].y, ((uint2 *) res)[1].x,
-                                          ((uint2 *) res)[1].y);
+        if constexpr (DXT_TYPE == 1 && BPT == 2) {  // the two blocks one phase apart (same operation tree per block)
+                const uint4 v[4] = { make_uint4(w[0][0], w[0][1], w[0][2], w[0][3]), make_uint4(w[1][0], w[1][1], w[1][2], w[1][3]),
+                                     make_uint4(w[2][0], w[2][1], w[2][2], w[2][3]), make_uint4(w[3][0], w[3][1], w[3][2], w[3][3]) };
+                *(uint4 *) o = dxt1_encode_uyvy_pair_skewed(v);
         } else {
 #pragma unroll
                 for (int k = 0; k < BPT; ++k) {
-                        o[k] = res[k];
+                        if constexpr (DXT_TYPE == 1) {  // paired formulation (same operation tree)
+                                const uint32_t wk[4][2] = { { w[0][2 * k], w[0][2 * k + 1] }, { w[1][2 * k], w[1][2 * k + 1] },
+                                                            { w[2][2 * k], w[2][2 * k + 1] }, { w[3][2 * k], w[3][2 * k + 1] } };
+                                o[k] = dxt1_encode_uyvy_packed(wk);
+                        } else {
+                                float r[16], g[16], b[16];
+#pragma unroll
+                                for (int y = 0; y < 4; ++y) {
+                                        load_row_uyvy_packed(w[y][2 * k], w[y][2 * k + 1], r + 4 * y, g + 4 * y, b + 4 * y);
+                                }
+                                o[k] = encode_block<DXT_TYPE>(r, g, b);
+                        }
                 }
         }
-}
-
-/// fused UYVY -> DXT1, two blocks per thread with their phases one apart (dxt1_encode_uyvy_pair_skewed): the ALU-only bounding box of one
-/// block between the FMA-only deviation / covariance / projection instructions of the other.  More live registers (both blocks' 48 colour
-/// values), hence fewer resident warps than dxt_uyvy_kernel<1, 2, .>; the kernel is not latency-bound (DESIGN.md section 4.2).
-template <bool MIRROR, int TPB, int MINB, int FINE = 0>  // FINE: 0 phases skewed, 1 statement-level alternation, 2 the same in basic blocks of one row
-__global__ void __launch_bounds__(TPB, MINB) dxt1_uyvy_skew_kernel(const uint8_t *__restrict__ src, void *__restrict__ out, int wb, int h, long pitch)
-{
-        const int gx = blockIdx.x * blockDim.x + threadIdx.x;
-        const int by = blockIdx.y;
-        if (gx >= wb / 2) {
-                return;
-        }
-        const int row0 = MIRROR ? h - 1 - by * 4 : by * 4;
-        const uint8_t *p = src + (long) row0 * pitch + gx * 16;
-        const long step = MIRROR ? -pitch : pitch;
-        uint4 v[4];
-#pragma unroll
-        for (int y = 0; y < 4; ++y, p += step) {
-                v[y] = ld_stream_v4(p);
-        }
-        *((uint4 *) out + ((long) by * (wb / 2) + gx)) =
-            FINE == 2 ? dxt1_encode_uyvy_pair_fine<true>(v, pitch) : FINE == 1 ? dxt1_encode_uyvy_pair_fine<false>(v, pitch) : dxt1_encode_uyvy_pair_skewed(v);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -317,8 +294,6 @@ static int launch_uyvy(const void *src, void *out, int sx, int sy, long pitch, c
 #define UGB_LAUNCH(BPT, MIR) dxt_uyvy_kernel<DXT_TYPE, BPT, MIR><<<grid, threads, 0, str>>>(s, out, wb, sy, pitch)
         if (DXT_TYPE == 1 && pair) {
                 if constexpr (DXT_TYPE == 1) {  // (the two-block variant is not even instantiated for DXT5-YCoCg)
-                        // (dxt1_uyvy_skew_kernel - the two blocks of a thread one phase apart - was no faster on an earlier GPU; it stays in this
-                        // file for tools/exp_dxt.cu only)
                         if (mirrored) {
                                 UGB_LAUNCH(2, true);
                         } else {
