@@ -7,6 +7,14 @@
  *   UGB_RGB  input -> R,G,B stored as-is, 4:4:4, THREE scans (non-interleaved), Adobe APP14 transform=0
  *   baseline sequential DCT (SOF0), Annex K Huffman tables, Annex K quantisation tables scaled by IJG quality,
  *   restart interval `restart_interval` MCUs (0 = default: 4 for UYVY, 8 for RGB — gpujpeg.cpp:351), RSTn markers.
+ * The _ex calls add what GPUJPEG's `subsampling` and internal colour space options ask for (gpujpeg.cpp:262-266,292-304,332):
+ *   UGB_I420 input (native 4:2:0, BT.709) -> YCbCr 4:2:0, one interleaved scan (MCU 16x16 = Y0 Y1 Y2 Y3 Cb Cr); the planes are read in place
+ *   UGB_UYVY input, subsampling 420          -> the same stream; chroma of two rows averaged as uyvy_to_i420 (to_planar.c:343-378)
+ *   UGB_RGB  input, Y709 | Y601 | Y601FULL   -> YCbCr 4:4:4 / 4:2:2 / 4:2:0 (subsampling 0 = 444), one scan per component (T.81 A.2: a
+ *                                               component's blocks are not padded to whole MCUs) or one interleaved scan with `interleaved`;
+ *                                               integer RGB_TO_Y/CB/CR of the reference at 8 bits (Y601FULL: JFIF full range)
+ *   every YCbCr stream carries JFIF APP0; restart interval default 8 for RGB input, 4 otherwise.  Native parameters give the bytes of
+ *   the calls without _ex.  Anything else returns -4: chroma upsampling, YCbCr -> RGB, one YCbCr matrix -> another, subsampled RGB.
  * Output capacity is width*height*3 + 4096 bytes like the reference's pool frames (gpujpeg.cpp:355).
  */
 #ifndef UGB200_JPEG_H
@@ -44,6 +52,17 @@ UGB_API void ugb200_jpeg_encoder_destroy(ugb200_jpeg_encoder *enc);
  * buffer, the capacity the reference gives libgpujpeg at gpujpeg.cpp:355 (noise at quality ~100 only). */
 UGB_API int ugb200_jpeg_encode_device(ugb200_jpeg_encoder *enc, const void *src, long pitch, int width, int height, int codec,
                                       const struct ugb200_jpeg_params *params);
+enum { UGB200_JPEG_CS_NATIVE = 0, UGB200_JPEG_CS_Y601, UGB200_JPEG_CS_Y601FULL, UGB200_JPEG_CS_Y709, UGB200_JPEG_CS_RGB };  /* = gpujpeg_opts::internal_cs */
+struct ugb200_jpeg_params_ex {
+        struct ugb200_jpeg_params base;
+        int subsampling;   /* 0 = native for the input (RGB 444, UYVY 422, I420 420), else 444 / 422 / 420 */
+        int color_space;   /* UGB200_JPEG_CS_* */
+};
+UGB_API void ugb200_jpeg_default_params_ex(struct ugb200_jpeg_params_ex *p);
+/* ugb200_jpeg_encode_device with the layouts above; `codec` also takes UGB_I420 (pitch must be 0) */
+UGB_API int ugb200_jpeg_encode_device_ex(ugb200_jpeg_encoder *enc, const void *src, long pitch, int width, int height, int codec,
+                                         const struct ugb200_jpeg_params_ex *params);
+
 /* Waits for the encode and returns the device pointer and byte size of the JPEG stream. */
 UGB_API int ugb200_jpeg_result_device(ugb200_jpeg_encoder *enc, const void **dev_ptr, size_t *size);
 
@@ -57,6 +76,10 @@ UGB_API int ugb200_jpeg_encode(ugb200_jpeg_encoder *enc, const void *src, int sr
  * -5 if the stream does not fit. */
 UGB_API int ugb200_jpeg_encode_into(ugb200_jpeg_encoder *enc, const void *src, int src_is_device, long pitch, int width, int height,
                                     int codec, const struct ugb200_jpeg_params *params, uint8_t *dst, size_t dst_cap, size_t *out_size);
+
+/* ugb200_jpeg_encode_into with the layouts of ugb200_jpeg_encode_device_ex; a host I420 source is vc_get_datalen bytes */
+UGB_API int ugb200_jpeg_encode_into_ex(ugb200_jpeg_encoder *enc, const void *src, int src_is_device, long pitch, int width, int height,
+                                       int codec, const struct ugb200_jpeg_params_ex *params, uint8_t *dst, size_t dst_cap, size_t *out_size);
 
 /* Measurement: with stage timing on, every encode records CUDA events between its kernels on the encoder's stream;
  * ugb200_jpeg_encoder_stage_times waits for the last encode and returns the device time in microseconds of

@@ -48,6 +48,18 @@ for codec, w, h, q, ri in ([] if ONLY == "staged" else ((2, 100, 52, 90, 0), (2,
         for out_c in (2, 12, 1, 29):
             dec.decode(s, out_c)
         n += 6
+# JPEG planar layouts (ugb200_jpeg_encode_device_ex) at ragged sizes, one per new row of the supported matrix: I420 read in place,
+# UYVY -> 4:2:0, RGB -> Y709 / Y601 / Y601full at 4:4:4 / 4:2:2 / 4:2:0, per-component and interleaved; the 4:2:0 streams decode to I420
+for codec, sub, cs, il in ([] if ONLY == "staged" else ((29, 0, 0, 1), (2, 420, 3, 1), (12, 0, 3, 0), (12, 422, 1, 1), (12, 420, 2, 0), (12, 420, 3, 1))):
+    for w, h, ri in ((17, 9, 3), (130, 37, 0)):
+        nbytes = w * h + 2 * ((w + 1) // 2) * ((h + 1) // 2) if codec == 29 else ((w + 1) // 2 * 4 if codec == 2 else w * 3) * h
+        src = torch.randint(0, 256, (nbytes,), dtype=torch.uint8, device="cuda")
+        enc.encode_device(src, w, h, codec, quality=90, restart_interval=ri, pitch=(w + 1) // 2 * 4 if codec == 2 else 0, interleaved=bool(il),
+                          subsampling=sub, color_space=cs)
+        s = enc.result()
+        if sub == 420 or codec == 29:
+            dec.decode(s, 29)
+        n += 2
 # round 2, state i: the staged launch forms of the line converters (16-byte aligned pitches, tight buffers), every form of every converter
 for inc, outc in ([] if ONLY == "jpeg" else PAIRS):
     for w, h in ((64, 2), (192, 3), (2048 + 64, 2)):

@@ -95,6 +95,9 @@ SIGNATURES = {
     "ugb200_jpeg_result_device": (_i, [_vp, ctypes.POINTER(_vp), ctypes.POINTER(_sz)]),
     "ugb200_jpeg_encode": (_i, [_vp, _vp, _i, _l, _i, _i, _i, _vp, ctypes.POINTER(_vp), ctypes.POINTER(_sz)]),
     "ugb200_jpeg_encode_into": (_i, [_vp, _vp, _i, _l, _i, _i, _i, _vp, _vp, _sz, ctypes.POINTER(_sz)]),
+    "ugb200_jpeg_default_params_ex": (None, [_vp]),
+    "ugb200_jpeg_encode_device_ex": (_i, [_vp, _vp, _l, _i, _i, _i, _vp]),
+    "ugb200_jpeg_encode_into_ex": (_i, [_vp, _vp, _i, _l, _i, _i, _i, _vp, _vp, _sz, ctypes.POINTER(_sz)]),
     "ugb200_jpeg_encoder_stage_timing": (_i, [_vp, _i]),
     "ugb200_jpeg_encoder_stage_times": (_i, [_vp, ctypes.POINTER(ctypes.c_float)]),
     "ugb200_jpeg_get_image_info": (_i, [_vp, _sz, _vp]),

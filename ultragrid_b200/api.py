@@ -217,6 +217,14 @@ class JpegParams(ctypes.Structure):
     _fields_ = [("quality", ctypes.c_int), ("restart_interval", ctypes.c_int), ("interleaved", ctypes.c_int)]
 
 
+class JpegParamsEx(ctypes.Structure):
+    """struct ugb200_jpeg_params_ex: subsampling 0 (native) / 444 / 422 / 420, color_space one of JPEG_CS"""
+    _fields_ = [("base", JpegParams), ("subsampling", ctypes.c_int), ("color_space", ctypes.c_int)]
+
+
+JPEG_CS = {"native": 0, "Y601": 1, "Y601full": 2, "Y709": 3, "RGB": 4}  # UGB200_JPEG_CS_* = gpujpeg_opts::internal_cs
+
+
 class JpegEncoder:
     """ugb200_jpeg_* (include/ugb200_jpeg.h): the stage src/video_compress/gpujpeg.cpp delegates to libgpujpeg."""
 
@@ -243,8 +251,24 @@ class JpegEncoder:
         p.interleaved = 1 if interleaved else 0
         return p
 
-    def encode_device(self, src, width, height, codec, quality=None, restart_interval=0, pitch=0, interleaved=False):
-        """asynchronous; returns nothing — call result() for the bytes"""
+    def _params_ex(self, quality, restart_interval, interleaved, subsampling, color_space):
+        p = JpegParamsEx()
+        _L.ugb200_jpeg_default_params_ex(ctypes.byref(p))
+        p.base = self._params(quality, restart_interval, interleaved)
+        p.subsampling, p.color_space = subsampling, color_space
+        return p
+
+    @staticmethod
+    def _use_ex(codec, subsampling, color_space):
+        """the _ex entry points only for what the plain ones cannot do: existing callers keep the calls they make"""
+        return bool(subsampling or color_space) or int(codec) == int(Codec.I420)
+
+    def encode_device(self, src, width, height, codec, quality=None, restart_interval=0, pitch=0, interleaved=False, subsampling=0, color_space=0):
+        """asynchronous; returns nothing — call result() for the bytes.  subsampling / color_space: see JpegParamsEx"""
+        if self._use_ex(codec, subsampling, color_space):
+            p = self._params_ex(quality, restart_interval, interleaved, subsampling, color_space)
+            _check(_L.ugb200_jpeg_encode_device_ex(self._h, _ptr(src), pitch, width, height, int(codec), ctypes.byref(p)), "ugb200_jpeg_encode_device_ex")
+            return
         p = self._params(quality, restart_interval, interleaved)
         _check(_L.ugb200_jpeg_encode_device(self._h, _ptr(src), pitch, width, height, int(codec), ctypes.byref(p)), "ugb200_jpeg_encode_device")
 
@@ -256,14 +280,21 @@ class JpegEncoder:
         _check(_L.cuda_wrapper_memcpy(host, ptr, n.value, 1), "cuda_wrapper_memcpy")
         return bytes(host)
 
-    def encode(self, src, width, height, codec, quality=None, restart_interval=0, pitch=0, interleaved=False):
+    def encode(self, src, width, height, codec, quality=None, restart_interval=0, pitch=0, interleaved=False, subsampling=0, color_space=0):
         """gpujpeg_encoder_encode: src is a host numpy array or a CUDA tensor; returns the JPEG bytes"""
-        p = self._params(quality, restart_interval, interleaved)
-        out, n = ctypes.c_void_p(), ctypes.c_size_t()
         if isinstance(src, torch.Tensor):
             sp, is_dev = _ptr(src), 1
         else:
             sp, is_dev = ctypes.c_void_p(src.ctypes.data), 0
+        if self._use_ex(codec, subsampling, color_space):
+            import numpy as np
+            p = self._params_ex(quality, restart_interval, interleaved, subsampling, color_space)
+            dst, n = np.empty(width * height * 3 + 4096, dtype=np.uint8), ctypes.c_size_t()
+            _check(_L.ugb200_jpeg_encode_into_ex(self._h, sp, is_dev, pitch, width, height, int(codec), ctypes.byref(p), ctypes.c_void_p(dst.ctypes.data),
+                                                 dst.size, ctypes.byref(n)), "ugb200_jpeg_encode_into_ex")
+            return dst[:n.value].tobytes()
+        p = self._params(quality, restart_interval, interleaved)
+        out, n = ctypes.c_void_p(), ctypes.c_size_t()
         _check(_L.ugb200_jpeg_encode(self._h, sp, is_dev, pitch, width, height, int(codec), ctypes.byref(p), ctypes.byref(out), ctypes.byref(n)),
                "ugb200_jpeg_encode")
         return ctypes.string_at(out.value, n.value)

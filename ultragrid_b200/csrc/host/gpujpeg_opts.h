@@ -3,9 +3,10 @@
 // src/video_compress/gpujpeg.cpp:371-424:
 //     <quality>[:<restart interval>] positionally, or quality=<n> (here also q=<n>), restart=<n>, interleaved, Y601 | Y601full | Y709 | RGB,
 //     subsampling=<444|422|420>, alpha; plus lanes=<n> (addition of this library: frames in flight per device).
-// This encoder stores the input as it comes (RGB input -> RGB, 4:4:4; UYVY input -> BT.709 YCbCr, 4:2:2 - the reference's own defaults, :295-305):
-// an internal colour space or a subsampling that would need a transform / resampling inside the codec is refused when the first frame shows the
-// input format (check_against_input), with a message instead of a silently different stream.
+// This module stores the input as it comes (RGB input -> RGB, 4:4:4; UYVY input -> BT.709 YCbCr, 4:2:2; I420 input -> BT.709 YCbCr, 4:2:0 - the
+// reference's own defaults, :295-305, :332): an internal colour space or a subsampling other than the input's own is refused when the first frame
+// shows the input format (check_against_input), with a message instead of a silently different stream.  The encoder itself can also convert
+// RGB to YCbCr and subsample chroma (ugb200_jpeg_encode_into_ex); opening those options here is a change of this policy only.
 #pragma once
 #include <cctype>
 #include <cstdio>
@@ -13,6 +14,8 @@
 #include <cstring>
 #include <string>
 #include <strings.h>
+
+enum class jpeg_input { UYVY, RGB, I420 };  // the encoder input formats
 
 struct gpujpeg_opts {
         int quality = -1;           // -1: encoder default (gpujpeg_set_default_parameters: 75)
@@ -100,23 +103,26 @@ struct gpujpeg_opts {
 
         static void usage()
         {
-                printf("GPUJPEG usage:\n\t-c GPUJPEG[:<quality>[:<restart_interval>]][:quality=<q>][:restart=<n>][:interleaved][:RGB|Y709][:subsampling=<444|422>][:lanes=<n>]\n"
+                printf("GPUJPEG usage:\n\t-c GPUJPEG[:<quality>[:<restart_interval>]][:quality=<q>][:restart=<n>][:interleaved][:RGB|Y709][:subsampling=<444|422|420>][:lanes=<n>]\n"
                        "\twhere\n\t\tinterleaved - one scan for RGB input too (default: one scan per component)\n"
                        "\t\tRGB|Y709 - must name the colour space the input already has (no transform inside the codec)\n"
+                       "\t\tsubsampling - must name the input's own: 444 for RGB, 422 for UYVY, 420 for I420 (I420 frames are encoded as they are)\n"
                        "\t\tlanes - frames in flight per CUDA device (default 3)\n");
         }
 
-        /// the options against the encoder input format (true RGB / false UYVY): what needs a transform inside the codec is refused
-        bool check_against_input(bool rgb_input) const
+        /// the options against the encoder input format: what needs a transform inside the codec is refused
+        bool check_against_input(jpeg_input in) const
         {
-                if (internal_cs != 0 && internal_cs != (rgb_input ? 4 : 3)) {
+                const char *name = in == jpeg_input::RGB ? "RGB" : in == jpeg_input::UYVY ? "UYVY" : "I420";
+                if (internal_cs != 0 && internal_cs != (in == jpeg_input::RGB ? 4 : 3)) {
                         fprintf(stderr, "[GPUJPEG] the requested internal colour space needs a colour transform inside the codec; this encoder stores %s input as %s\n",
-                                rgb_input ? "RGB" : "UYVY", rgb_input ? "RGB" : "BT.709 YCbCr");
+                                name, in == jpeg_input::RGB ? "RGB" : "BT.709 YCbCr");
                         return false;
                 }
-                if (subsampling != 0 && subsampling != (rgb_input ? 444 : 422)) {
-                        fprintf(stderr, "[GPUJPEG] subsampling=%d needs resampling inside the codec; %s input is stored as 4:%s\n", subsampling, rgb_input ? "RGB" : "UYVY",
-                                rgb_input ? "4:4" : "2:2");
+                const int native = in == jpeg_input::RGB ? 444 : in == jpeg_input::UYVY ? 422 : 420;
+                if (subsampling != 0 && subsampling != native) {
+                        fprintf(stderr, "[GPUJPEG] subsampling=%d needs resampling inside the codec; %s input is stored as 4:%s\n", subsampling, name,
+                                native == 444 ? "4:4" : native == 422 ? "2:2" : "2:0");
                         return false;
                 }
                 if (alpha) {

@@ -485,11 +485,13 @@ std::shared_ptr<video_frame> encoder_state::compress_step(std::shared_ptr<video_
         const struct video_desc desc = video_desc_from_frame(tx.get());
         if (!video_desc_eq(desc, saved_desc)) {  // configure_with, :256-369
                 const codec_t supported[] = { UYVY, RGB, VIDEO_CODEC_NONE };
-                if (!get_best_decoder_from(desc.color_spec, supported, &enc_input_codec)) {
+                if (desc.color_spec == I420) {  // planar I420 goes into the encoder as it is (gpujpeg.cpp:262-266)
+                        enc_input_codec = I420;
+                } else if (!get_best_decoder_from(desc.color_spec, supported, &enc_input_codec)) {
                         fprintf(stderr, "[GPUJPEG] Unsupported codec: %s\n", get_codec_name(desc.color_spec));
                         return {};
                 }
-                if (!parent->opts.check_against_input(enc_input_codec == RGB)) {
+                if (!parent->opts.check_against_input(enc_input_codec == RGB ? jpeg_input::RGB : enc_input_codec == I420 ? jpeg_input::I420 : jpeg_input::UYVY)) {
                         return {};
                 }
                 saved_desc = desc;
@@ -532,13 +534,15 @@ std::shared_ptr<video_frame> encoder_state::compress_step(std::shared_ptr<video_
                 }
                 in = cuda_conv;
         }
-        struct ugb200_jpeg_params p;
-        ugb200_jpeg_default_params(&p);
+        struct ugb200_jpeg_params_ex p;
+        ugb200_jpeg_default_params_ex(&p);
         if (parent->opts.quality != -1) {
-                p.quality = parent->opts.quality;
+                p.base.quality = parent->opts.quality;
         }
-        p.restart_interval = parent->opts.restart_interval;
-        p.interleaved = parent->opts.interleaved ? 1 : 0;
+        p.base.restart_interval = parent->opts.restart_interval;
+        p.base.interleaved = parent->opts.interleaved ? 1 : 0;
+        p.subsampling = parent->opts.subsampling;  // as checked against the input: the input's own layout
+        p.color_space = parent->opts.internal_cs;
         // the stream goes straight into the pooled (pinned) output frame: no encoder-owned buffer + memcpy as at :629-630
         const size_t out_cap = (size_t) w * h * 3 + 4096;  // :355 plus the header allowance of the encoder's own buffer (ugb200_jpeg.h): tiny or
                                                            // noisy frames at high quality exceed the raw size by their ~600-byte header
@@ -547,7 +551,7 @@ std::shared_ptr<video_frame> encoder_state::compress_step(std::shared_ptr<video_
                 return {};
         }
         size_t size = 0;
-        if (ugb200_jpeg_encode_into(encoder, in, 1, 0, (int) w, (int) h, enc_input_codec, &p, (uint8_t *) out->tiles[0].data, out_cap, &size) != 0) {  // :624
+        if (ugb200_jpeg_encode_into_ex(encoder, in, 1, 0, (int) w, (int) h, enc_input_codec, &p, (uint8_t *) out->tiles[0].data, out_cap, &size) != 0) {  // :624
                 return {};
         }
         out->color_spec = JPEG, out->fps = tx->fps, out->interlacing = tx->interlacing;

@@ -20,13 +20,16 @@
 
 #include "../../include/ugb200.h"
 #include "../../include/ugb200_jpeg.h"
+#include "color_space.h"
 #include "jpeg_compact.cuh"
 #include "f32x2.cuh"
 #include "jpeg_tables.h"
 
 namespace ugb {
 
-enum { FMT_UYVY_422 = 0, FMT_RGB_444 = 1 };
+// FMT_PLANAR: three 8-bit planes (I420 read in place, or the planes jpeg_prep_kernel writes), a YCbCr stream with luma sampled
+// 1x1, 2x1 or 2x2 and chroma 1x1; it always takes the split path (an interleaved 4:2:0 MCU has 6 blocks)
+enum { FMT_UYVY_422 = 0, FMT_RGB_444 = 1, FMT_PLANAR = 2 };
 constexpr int kSlotBytesPerBlock = 416;  // worst case: 1658 bits/block = 208 B, every byte stuffed
 constexpr int kSlotExtra = 8;            // final pad byte + RSTn
 
@@ -56,6 +59,20 @@ struct jpeg_geom {
         int header_len;    // bytes before the first entropy-coded byte (including the first SOS)
         int sos_len;       // length of one later SOS header (RGB)
         int interleaved;   // RGB only: one scan, MCU = the R, G and B block of an 8x8 area (GPUJPEG's `interleaved` option, gpujpeg.cpp:303)
+};
+
+// Scan table of every stream (the offset scan and the compaction read it) and the geometry of FMT_PLANAR.  Kept out of jpeg_geom, which
+// the fused kernel takes: its code stays exactly as it was.
+struct jpeg_layout {
+        int nscans;        // scans in the stream
+        int scan_seg0[4];  // first segment of each scan; the entries from nscans on hold nseg
+        // FMT_PLANAR only
+        int hs, vs;                  // luma sampling factors (chroma is 1x1)
+        int scan_mcus[3];            // MCUs of each scan
+        int comp_bw[3], comp_blk0[3];  // non-interleaved: blocks per row of each component (T.81 A.2) and its first block in scan order
+        int plane_w[3], plane_h[3];  // valid samples of each plane (edges replicate the last column / row)
+        long plane_pitch[3];
+        const uint8_t *plane[3];
 };
 
 // ---- K1 -------------------------------------------------------------------------------------------------------------
@@ -130,12 +147,52 @@ __device__ __forceinline__ void load_row(const uint8_t *__restrict__ src, long p
         }
 }
 
+/// 8 samples of one row of a block of plane `comp` (FMT_PLANAR); interior: 8-byte aligned and inside the plane
+__device__ __forceinline__ void load_row_planar(const jpeg_layout &L, int comp, int bx, int y, bool interior, float *f)
+{
+        const uint8_t *plane = comp == 0 ? L.plane[0] : comp == 1 ? L.plane[1] : L.plane[2];
+        const long pitch = comp == 0 ? L.plane_pitch[0] : comp == 1 ? L.plane_pitch[1] : L.plane_pitch[2];
+        const int pw = comp == 0 ? L.plane_w[0] : L.plane_w[1], ph = comp == 0 ? L.plane_h[0] : L.plane_h[1];
+        const uint8_t *row = plane + (long) clampi(y, ph - 1) * pitch;
+        if (interior) {
+                const uint2 v = __ldg((const uint2 *) (row + (long) bx * 8));
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                        f[i] = shifted(v.x, i);
+                        f[4 + i] = shifted(v.y, i);
+                }
+        } else {
+#pragma unroll
+                for (int x = 0; x < 8; ++x) {
+                        f[x] = shifted((uint32_t) __ldg(row + clampi(bx * 8 + x, pw - 1)), 0);
+                }
+        }
+}
+
+/// PLANAR: FMT_PLANAR geometry (a template flag, so that the UYVY / RGB instantiation keeps its code)
+template <bool PLANAR>
 __global__ void __launch_bounds__(128) jpeg_dct_kernel(const uint8_t *__restrict__ src, long pitch, jpeg_geom g, int16_t *__restrict__ coef,
-                                                       bool vec_ok, const __grid_constant__ jpeg_qtab qt)
+                                                       bool vec_ok, const __grid_constant__ jpeg_qtab qt, const __grid_constant__ jpeg_layout L)
 {
         int b = blockIdx.x * blockDim.x + threadIdx.x;
         int comp, bx, by;
-        if (g.fmt == FMT_UYVY_422) {
+        if (PLANAR) {
+                if (b >= g.nblocks) {
+                        return;
+                }
+                if (g.interleaved) {  // MCU = hs x vs luma blocks in raster order, then Cb, Cr (T.81 A.2.3)
+                        const int nl = L.hs * L.vs, m = b / g.blocks_per_mcu, k = b - m * g.blocks_per_mcu;
+                        const int mx = m % g.bw, my = m / g.bw;
+                        comp = k < nl ? 0 : k - nl + 1;
+                        bx = k < nl ? mx * L.hs + k % L.hs : mx;
+                        by = k < nl ? my * L.vs + k / L.hs : my;
+                } else {  // one scan per component, each in raster order of its own block grid
+                        comp = b >= L.comp_blk0[2] ? 2 : b >= L.comp_blk0[1] ? 1 : 0;
+                        const int r = b - (comp == 0 ? 0 : comp == 1 ? L.comp_blk0[1] : L.comp_blk0[2]);
+                        const int cbw = comp == 0 ? L.comp_bw[0] : comp == 1 ? L.comp_bw[1] : L.comp_bw[2];
+                        bx = r % cbw, by = r / cbw;
+                }
+        } else if (g.fmt == FMT_UYVY_422) {
                 // a CTA of 4 warps owns 32 MCUs; warp k encodes block k (Y0, Y1, Cb, Cr) of each, so that a warp is
                 // component-uniform: no luma/chroma divergence, uniform constant-bank reads of the quantiser table
                 const int k = threadIdx.x >> 5, m = blockIdx.x * 32 + (threadIdx.x & 31);
@@ -163,12 +220,21 @@ __global__ void __launch_bounds__(128) jpeg_dct_kernel(const uint8_t *__restrict
                 }
         }
         // interior: the whole block lies inside the image (and vector loads are aligned)
-        const int px_w = (g.fmt == FMT_UYVY_422 && comp != 0) ? 16 : 8;
-        const bool interior = vec_ok && (bx + 1) * px_w <= g.w && (by + 1) * 8 <= g.h;
         float f[64];
+        if (PLANAR) {
+                const int pw = comp == 0 ? L.plane_w[0] : L.plane_w[1], ph = comp == 0 ? L.plane_h[0] : L.plane_h[1];
+                const bool interior = vec_ok && (bx + 1) * 8 <= pw && (by + 1) * 8 <= ph;
 #pragma unroll
-        for (int y = 0; y < 8; ++y) {
-                load_row(src, pitch, g, comp, bx, by * 8 + y, interior, f + 8 * y);
+                for (int y = 0; y < 8; ++y) {
+                        load_row_planar(L, comp, bx, by * 8 + y, interior, f + 8 * y);
+                }
+        } else {
+                const int px_w = (g.fmt == FMT_UYVY_422 && comp != 0) ? 16 : 8;
+                const bool interior = vec_ok && (bx + 1) * px_w <= g.w && (by + 1) * 8 <= g.h;
+#pragma unroll
+                for (int y = 0; y < 8; ++y) {
+                        load_row(src, pitch, g, comp, bx, by * 8 + y, interior, f + 8 * y);
+                }
         }
 #pragma unroll
         for (int r = 0; r < 8; ++r) {
@@ -1262,9 +1328,12 @@ __global__ void __launch_bounds__(128) jpeg_assemble_kernel(jpeg_geom g, const u
 /// One thread per restart segment.  Per block: 8 x LDG.128 build a 64-bit non-zero map (uniform work), then the loop runs once
 /// per NON-ZERO coefficient (ffs over the map) instead of once per coefficient — far less divergence inside a warp.
 /// The CTA also produces the exclusive prefix of its 128 segment sizes and its total (first level of the stream scan).
+/// PLANAR: FMT_PLANAR geometry (scans of different lengths; luma blocks per MCU from the sampling factors)
+template <bool PLANAR>
 __global__ void __launch_bounds__(128) jpeg_huffman_kernel(const int16_t *__restrict__ coef, jpeg_geom g, uint8_t *__restrict__ slots,
                                                            uint32_t *__restrict__ sizes, uint32_t *__restrict__ local_off,
-                                                           uint32_t *__restrict__ cta_total, const uint32_t *__restrict__ huff)
+                                                           uint32_t *__restrict__ cta_total, const uint32_t *__restrict__ huff,
+                                                           const __grid_constant__ jpeg_layout L)
 {
         __shared__ uint32_t s_dc[2][16], s_ac[2][256], s_warp[4];
         for (int i = threadIdx.x; i < 32; i += blockDim.x) {
@@ -1277,8 +1346,18 @@ __global__ void __launch_bounds__(128) jpeg_huffman_kernel(const int16_t *__rest
         const int s = blockIdx.x * blockDim.x + threadIdx.x;
         uint32_t nbytes = 0;
         if (s < g.nseg) {
-                const int scan = s / g.seg_per_scan, ls = s - scan * g.seg_per_scan;
-                const int m0 = ls * g.ri, m1 = min(m0 + g.ri, g.mcu_per_scan);
+                int scan, ls, segs, mcus;
+                if (PLANAR) {
+                        scan = (s >= L.scan_seg0[1]) + (s >= L.scan_seg0[2]);
+                        const int s0 = scan == 0 ? 0 : scan == 1 ? L.scan_seg0[1] : L.scan_seg0[2];
+                        ls = s - s0;
+                        segs = (scan == 0 ? L.scan_seg0[1] : scan == 1 ? L.scan_seg0[2] : L.scan_seg0[3]) - s0;
+                        mcus = scan == 0 ? L.scan_mcus[0] : scan == 1 ? L.scan_mcus[1] : L.scan_mcus[2];
+                } else {
+                        scan = s / g.seg_per_scan, ls = s - scan * g.seg_per_scan;
+                        segs = g.seg_per_scan, mcus = g.mcu_per_scan;
+                }
+                const int m0 = ls * g.ri, m1 = min(m0 + g.ri, mcus);
                 uint32_t *base = (uint32_t *) (slots + (long) s * g.slot);
                 bit_writer bw = { base, 0, 0, 0, 0 };
                 int pred[3] = { 0, 0, 0 };
@@ -1286,7 +1365,12 @@ __global__ void __launch_bounds__(128) jpeg_huffman_kernel(const int16_t *__rest
                         for (int k = 0; k < g.blocks_per_mcu; ++k) {
                                 int comp;
                                 long blk;
-                                if (g.fmt == FMT_UYVY_422) {
+                                if (PLANAR) {
+                                        const int nl = g.blocks_per_mcu - 2;
+                                        comp = !g.interleaved ? scan : k < nl ? 0 : k - nl + 1;
+                                        blk = !g.interleaved ? (long) (scan == 0 ? 0 : scan == 1 ? L.comp_blk0[1] : L.comp_blk0[2]) + m
+                                                             : (long) m * g.blocks_per_mcu + k;
+                                } else if (g.fmt == FMT_UYVY_422) {
                                         comp = k < 2 ? 0 : k - 1;
                                         blk = (long) m * 4 + k;
                                 } else if (g.interleaved) {
@@ -1346,7 +1430,7 @@ __global__ void __launch_bounds__(128) jpeg_huffman_kernel(const int16_t *__rest
                         }
                 }
                 bw.flush_bits();
-                if (ls != g.seg_per_scan - 1) {  // RSTn between segments of a scan
+                if (ls != segs - 1) {  // RSTn between segments of a scan
                         bw.emit_byte(0xFF);
                         bw.emit_byte(0xD0 + (ls & 7));
                 }
@@ -1382,7 +1466,7 @@ __global__ void __launch_bounds__(128) jpeg_huffman_kernel(const int16_t *__rest
 // ---- K3: exclusive scan of the per-CTA totals (second level; a frame has 8 100 - 36 450 of them) ------------------------------------
 // One CTA of 1024 threads, eight consecutive totals per thread and round (two 128-bit loads, thread-local prefix, one block scan of the
 // thread sums): an 8K UYVY frame is ONE round.
-__global__ void __launch_bounds__(1024) jpeg_scan_kernel(uint32_t *__restrict__ cta_total, int n, jpeg_geom g, uint32_t *__restrict__ total)
+__global__ void __launch_bounds__(1024) jpeg_scan_kernel(uint32_t *__restrict__ cta_total, int n, jpeg_geom g, uint32_t *__restrict__ total, int nscans)
 {
         __shared__ uint32_t s_warp[32];
         __shared__ uint32_t s_carry;
@@ -1442,7 +1526,6 @@ __global__ void __launch_bounds__(1024) jpeg_scan_kernel(uint32_t *__restrict__ 
                 __syncthreads();
         }
         if (threadIdx.x == 0) {
-                const int nscans = g.nseg / g.seg_per_scan;
                 *total = g.header_len + carry + g.sos_len * (nscans - 1) + 2;  // + later SOS headers + EOI
         }
 }
@@ -1456,7 +1539,7 @@ constexpr int kCompactLanes = 8;
 __global__ void __launch_bounds__(256) jpeg_compact_kernel(const uint8_t *__restrict__ slots, const uint32_t *__restrict__ sizes,
                                                            const uint32_t *__restrict__ local_off, const uint32_t *__restrict__ cta_base,
                                                            jpeg_geom g, int segs_per_cta, int ctas_per_scan, uint8_t *__restrict__ out,
-                                                           const uint32_t *__restrict__ total, uint32_t out_cap)
+                                                           const uint32_t *__restrict__ total, uint32_t out_cap, const __grid_constant__ jpeg_layout L)
 {
         const int t = blockIdx.x * blockDim.x + threadIdx.x;
         const int s = t / kCompactLanes, lane = t % kCompactLanes;
@@ -1464,12 +1547,13 @@ __global__ void __launch_bounds__(256) jpeg_compact_kernel(const uint8_t *__rest
         if (s >= g.nseg || *total > out_cap) {  // a stream larger than the output buffer is reported by the host, never written
                 return;
         }
-        const int scan = s / g.seg_per_scan;
+        const int scan = (s >= L.scan_seg0[1]) + (s >= L.scan_seg0[2]);  // scans may differ in length (4:2:0: the Y scan has 4x the blocks)
+        const int seg0 = scan == 0 ? 0 : scan == 1 ? L.scan_seg0[1] : L.scan_seg0[2];
         // which CTA of the entropy kernel produced this segment: split path = 128 consecutive segments; fused path = per scan
-        const int cta = ctas_per_scan ? scan * ctas_per_scan + (s - scan * g.seg_per_scan) / segs_per_cta : s / segs_per_cta;
+        const int cta = ctas_per_scan ? scan * ctas_per_scan + (s - seg0) / segs_per_cta : s / segs_per_cta;
         const uint32_t n = sizes[s], off = g.header_len + cta_base[cta] + local_off[s] + g.sos_len * scan;
         compact_segment(lane, kCompactLanes, (const uint32_t *) (slots + (long) s * g.slot), n, out + off);  // g.slot is a multiple of 8
-        if (lane == 0 && s > 0 && s % g.seg_per_scan == 0) {  // SOS header of a later scan (RGB: one component per scan)
+        if (lane == 0 && s > 0 && s == seg0) {  // SOS header of a later scan (one component per scan)
                 uint8_t *h = out + off - g.sos_len;
                 const uint8_t sos[10] = { 0xFF, 0xDA, 0, 8, 1, (uint8_t) (scan + 1), 0x11, 0, 63, 0 };
                 for (int i = 0; i < 10; ++i) {
@@ -1479,6 +1563,72 @@ __global__ void __launch_bounds__(256) jpeg_compact_kernel(const uint8_t *__rest
         if (lane == 0 && s == g.nseg - 1) {
                 out[off + n] = 0xFF, out[off + n + 1] = 0xD9;  // EOI
         }
+}
+
+// ---- pre-processing of the planar path: packed input -> the encoder's planes -------------------------------------------------
+// Integer arithmetic only, restated by the test oracle byte for byte:
+//   RGB:  Y = ((y_r R + y_g G + y_b B) >> 14) + off_y, Cb / Cr = (... >> 14) + 128 - the RGB_TO_* expressions of the reference's
+//         rgb_to_yuv444p (to_lavc_vid_conv.c:1206-1214) at 8 bits; >> is a floor division.  Every result lies in 0..255 for the three
+//         coefficient sets used (checked over the whole RGB cube by the tests), so nothing is clamped.  Subsampled chroma is the
+//         rounded mean of the full-resolution values: (a + b + 1) >> 1 of a pair (4:2:2), (a + b + c + d + 2) >> 2 of a quad (4:2:0);
+//         a missing last column or row takes its neighbour's value.
+//   UYVY -> 4:2:0: uyvy_to_i420 (to_planar.c:343-378): Cb / Cr = (a + b + 1) / 2 of two rows, the last row paired with itself.
+// what jpeg_prep_kernel does: nothing (I420 planes are read in place), UYVY -> 4:2:0, or RGB -> YCbCr with the coefficients of
+// PREP_RGB + UGB200_JPEG_CS_{Y601,Y601FULL,Y709}
+enum { PREP_NONE = 0, PREP_UYVY = 1, PREP_RGB = 2 };
+struct jpeg_prep_args {
+        const uint8_t *src;
+        long pitch;
+        int w, h;
+        int rgb;       // 1 packed RGB, 0 UYVY (4:2:0 only)
+        int hs, vs;    // luma samples per chroma sample
+        int c[9];      // y_r y_g y_b cb_r cb_g cb_b cr_r cr_g cr_b (Q14)
+        int off_y;
+        int cw, ch;    // chroma plane size
+        uint8_t *p[3];
+        long pp[3];
+};
+
+__global__ void __launch_bounds__(256) jpeg_prep_kernel(const __grid_constant__ jpeg_prep_args a)
+{
+        const long i = (long) blockIdx.x * blockDim.x + threadIdx.x;  // one thread per chroma sample
+        if (i >= (long) a.cw * a.ch) {
+                return;
+        }
+        const int cx = (int) (i % a.cw), cy = (int) (i / a.cw);
+        if (!a.rgb) {
+                const int y0 = 2 * cy, y1 = min(y0 + 1, a.h - 1), x0 = 2 * cx;
+                const uint8_t *r0 = a.src + (long) y0 * a.pitch + 4 * cx, *r1 = a.src + (long) y1 * a.pitch + 4 * cx;
+                const uchar4 u = make_uchar4(r0[0], r0[1], r0[2], r0[3]), v = make_uchar4(r1[0], r1[1], r1[2], r1[3]);  // any pitch
+                a.p[1][(long) cy * a.pp[1] + cx] = (uint8_t) ((u.x + v.x + 1) / 2);
+                a.p[2][(long) cy * a.pp[2] + cx] = (uint8_t) ((u.z + v.z + 1) / 2);
+                uint8_t *o0 = a.p[0] + (long) y0 * a.pp[0] + x0, *o1 = a.p[0] + (long) y1 * a.pp[0] + x0;
+                o0[0] = u.y, o1[0] = v.y;
+                if (x0 + 1 < a.w) {
+                        o0[1] = u.w, o1[1] = v.w;
+                }
+                return;
+        }
+        int sb = 0, sr = 0;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+#pragma unroll
+                for (int k = 0; k < 2; ++k) {
+                        if (j < a.vs && k < a.hs) {
+                                const int x = cx * a.hs + k, y = cy * a.vs + j;
+                                const uint8_t *px = a.src + (long) min(y, a.h - 1) * a.pitch + 3 * (long) min(x, a.w - 1);
+                                const int R = px[0], G = px[1], B = px[2];
+                                if (x < a.w && y < a.h) {
+                                        a.p[0][(long) y * a.pp[0] + x] = (uint8_t) (((a.c[0] * R + a.c[1] * G + a.c[2] * B) >> 14) + a.off_y);
+                                }
+                                sb += ((a.c[3] * R + a.c[4] * G + a.c[5] * B) >> 14) + 128;
+                                sr += ((a.c[6] * R + a.c[7] * G + a.c[8] * B) >> 14) + 128;
+                        }
+                }
+        }
+        const int n = a.hs * a.vs, sh = n == 1 ? 0 : n == 2 ? 1 : 2;  // n = 1, 2 or 4
+        a.p[1][(long) cy * a.pp[1] + cx] = (uint8_t) ((sb + (n >> 1)) >> sh);
+        a.p[2][(long) cy * a.pp[2] + cx] = (uint8_t) ((sr + (n >> 1)) >> sh);
 }
 
 }  // namespace ugb
@@ -1491,8 +1641,11 @@ using namespace ugb;
 struct ugb200_jpeg_encoder {
         cudaStream_t stream = nullptr;
         // cached configuration
-        int fmt = -1, w = 0, h = 0, quality = -1, ri = -1, interleaved = -1;
+        int fmt = -1, w = 0, h = 0, quality = -1, ri = -1, interleaved = -1, hs = 0, vs = 0, prep = -1;
         jpeg_geom g{};
+        jpeg_layout lay{};
+        uint8_t *planes = nullptr;  // FMT_PLANAR from packed input: jpeg_prep_kernel's output
+        size_t planes_cap = 0;
         std::vector<uint8_t> header;
         // device buffers
         int16_t *coef = nullptr;
@@ -1595,7 +1748,7 @@ void build_header(ugb200_jpeg_encoder *e, const uint8_t ql[64], const uint8_t qc
         v.push_back(3);
         for (int c = 0; c < 3; ++c) {
                 v.push_back((uint8_t) (c + 1));
-                v.push_back((e->fmt == FMT_UYVY_422 && c == 0) ? 0x21 : 0x11);
+                v.push_back(c != 0 ? 0x11 : e->fmt == FMT_UYVY_422 ? 0x21 : e->fmt == FMT_PLANAR ? (uint8_t) (e->hs << 4 | e->vs) : 0x11);
                 v.push_back(c == 0 ? 0 : 1);
         }
         put_dht(v, 0x00, ugb_jpeg_dc_luma_bits, ugb_jpeg_dc_vals, 12);
@@ -1615,9 +1768,14 @@ void build_header(ugb200_jpeg_encoder *e, const uint8_t ql[64], const uint8_t qc
         v.push_back(0), v.push_back(63), v.push_back(0);
 }
 
-int configure(ugb200_jpeg_encoder *e, int fmt, int w, int h, int quality, int ri, int interleaved)
+/// FMT_PLANAR: hs x vs luma sampling, the caller resolves `interleaved` and the restart interval; `prep` = what jpeg_prep_kernel does
+/// (PREP_*), part of the cache key like the geometry
+int configure(ugb200_jpeg_encoder *e, int fmt, int w, int h, int quality, int ri, int interleaved, int hs = 1, int vs = 1, int prep = PREP_NONE)
 {
-        interleaved = fmt == FMT_RGB_444 && interleaved ? 1 : 0;  // a UYVY stream is one interleaved scan anyway
+        if (fmt != FMT_PLANAR) {
+                interleaved = fmt == FMT_RGB_444 && interleaved ? 1 : 0;  // a UYVY stream is one interleaved scan anyway
+                hs = vs = 1, prep = PREP_NONE;
+        }
         if (ri <= 0) {
                 ri = fmt == FMT_RGB_444 ? 8 : 4;  // src/video_compress/gpujpeg.cpp:351
         }
@@ -1625,14 +1783,56 @@ int configure(ugb200_jpeg_encoder *e, int fmt, int w, int h, int quality, int ri
                 return -1;
         }
         quality = quality < 1 ? 1 : quality > 100 ? 100 : quality;
-        const bool same = e->fmt == fmt && e->w == w && e->h == h && e->quality == quality && e->ri == ri && e->interleaved == interleaved;
+        const bool same = e->fmt == fmt && e->w == w && e->h == h && e->quality == quality && e->ri == ri && e->interleaved == interleaved &&
+                          e->hs == hs && e->vs == vs && e->prep == prep;
         if (same) {
                 return 0;
         }
-        e->fmt = fmt, e->w = w, e->h = h, e->quality = quality, e->ri = ri, e->interleaved = interleaved;
+        e->fmt = fmt, e->w = w, e->h = h, e->quality = quality, e->ri = ri, e->interleaved = interleaved, e->hs = hs, e->vs = vs, e->prep = prep;
         jpeg_geom &g = e->g;
+        jpeg_layout &L = e->lay;
+        g = jpeg_geom{}, L = jpeg_layout{};
         g.fmt = fmt, g.w = w, g.h = h, g.ri = ri, g.interleaved = interleaved;
-        if (fmt == FMT_UYVY_422) {
+        L.hs = hs, L.vs = vs;
+        if (fmt == FMT_PLANAR) {
+                const int cw = (w + hs - 1) / hs, ch = (h + vs - 1) / vs;  // T.81 A.1.1: chroma is ceil(w * 1 / hs) x ceil(h * 1 / vs)
+                L.plane_w[0] = w, L.plane_h[0] = h;
+                for (int c = 1; c < 3; ++c) {
+                        L.plane_w[c] = cw, L.plane_h[c] = ch;
+                }
+                if (interleaved) {  // one scan; MCU = hs x vs luma blocks + Cb + Cr over an (8 hs) x (8 vs) area
+                        g.bw = (w + 8 * hs - 1) / (8 * hs), g.bh = (h + 8 * vs - 1) / (8 * vs);
+                        g.mcu_per_scan = g.bw * g.bh, g.blocks_per_mcu = hs * vs + 2;
+                        g.nblocks = g.mcu_per_scan * g.blocks_per_mcu;
+                        g.seg_per_scan = (g.mcu_per_scan + ri - 1) / ri;
+                        g.nseg = g.seg_per_scan, L.nscans = 1, g.sos_len = 0;
+                        L.scan_mcus[0] = g.mcu_per_scan;
+                } else {  // one scan per component; MCU = one block; each component's block grid is not padded to whole MCUs (T.81 A.2.2)
+                        g.blocks_per_mcu = 1, L.nscans = 3, g.sos_len = 10, g.nblocks = 0, g.nseg = 0;
+                        for (int c = 0; c < 3; ++c) {
+                                L.comp_bw[c] = (L.plane_w[c] + 7) / 8;
+                                L.comp_blk0[c] = g.nblocks;
+                                L.scan_mcus[c] = L.comp_bw[c] * ((L.plane_h[c] + 7) / 8);
+                                L.scan_seg0[c] = g.nseg;
+                                g.nblocks += L.scan_mcus[c];
+                                g.nseg += (L.scan_mcus[c] + ri - 1) / ri;
+                        }
+                        g.bw = L.comp_bw[0], g.bh = (h + 7) / 8, g.mcu_per_scan = L.scan_mcus[0];
+                        g.seg_per_scan = (g.mcu_per_scan + ri - 1) / ri;
+                }
+                for (int c = L.nscans; c < 4; ++c) {
+                        L.scan_seg0[c] = g.nseg;
+                }
+                if (prep != PREP_NONE) {  // planes written by jpeg_prep_kernel: 16-byte aligned rows, 256-byte aligned planes
+                        const long py = (w + 15) & ~15, pc = (cw + 15) & ~15;
+                        const size_t oc = ((size_t) py * h + 255) & ~(size_t) 255, oc2 = oc + (((size_t) pc * ch + 255) & ~(size_t) 255);
+                        if (!grow(e->planes, e->planes_cap, oc2 + (size_t) pc * ch)) {
+                                return -2;
+                        }
+                        L.plane[0] = e->planes, L.plane[1] = e->planes + oc, L.plane[2] = e->planes + oc2;
+                        L.plane_pitch[0] = py, L.plane_pitch[1] = L.plane_pitch[2] = pc;
+                }
+        } else if (fmt == FMT_UYVY_422) {
                 g.bw = (w + 15) / 16, g.bh = (h + 7) / 8;
                 g.mcu_per_scan = g.bw * g.bh, g.blocks_per_mcu = 4;
                 g.nblocks = g.mcu_per_scan * 4;
@@ -1649,6 +1849,12 @@ int configure(ugb200_jpeg_encoder *e, int fmt, int w, int h, int quality, int ri
                 if (interleaved) {  // one scan of R G B MCUs
                         g.blocks_per_mcu = 3;
                         g.nseg = g.seg_per_scan, g.sos_len = 0;
+                }
+        }
+        if (fmt != FMT_PLANAR) {  // scans of equal length
+                L.nscans = g.nseg / g.seg_per_scan;
+                for (int c = 0; c < 4; ++c) {
+                        L.scan_seg0[c] = min(c, L.nscans) * g.seg_per_scan;
                 }
         }
         g.slot = ri * g.blocks_per_mcu * kSlotBytesPerBlock + kSlotExtra;
@@ -1732,7 +1938,7 @@ void ugb200_jpeg_encoder_destroy(ugb200_jpeg_encoder *e)
         cudaStreamSynchronize(e->stream);
         cudaFree(e->coef), cudaFree(e->slots), cudaFree(e->out), cudaFree(e->staging);
         cudaFree(e->sizes), cudaFree(e->offsets), cudaFree(e->cta_total), cudaFree(e->total), cudaFree(e->lb_state), cudaFree(e->d_huff);
-        cudaFree(e->gbits), cudaFree(e->glen);
+        cudaFree(e->gbits), cudaFree(e->glen), cudaFree(e->planes);
         cudaFreeHost(e->h_out), cudaFreeHost(e->h_in), cudaFreeHost(e->h_total);
         if (e->stats_ev) {
                 cudaEventDestroy(e->stats_ev);
@@ -1754,6 +1960,8 @@ static void adapt_cap(ugb200_jpeg_encoder *e)
         }
         e->stats_pending = false;
 }
+
+static int launch_tail(ugb200_jpeg_encoder *e, int nctas, int segs_per_cta, int ctas_per_scan, bool single_pass, bool two_kernels);
 
 int ugb200_jpeg_encode_device(ugb200_jpeg_encoder *e, const void *src, long pitch, int width, int height, int codec,
                               const struct ugb200_jpeg_params *params)
@@ -1897,10 +2105,17 @@ int ugb200_jpeg_encode_device(ugb200_jpeg_encoder *e, const void *src, long pitc
                 }
         } else {  // split path: any restart interval
                 const int dct_ctas = fmt == FMT_UYVY_422 ? (g.mcu_per_scan + 31) / 32 : (g.nblocks + 127) / 128;
-                jpeg_dct_kernel<<<dct_ctas, 128, 0, e->stream>>>((const uint8_t *) src, pitch, g, e->coef, vec_ok, e->qt);
+                jpeg_dct_kernel<false><<<dct_ctas, 128, 0, e->stream>>>((const uint8_t *) src, pitch, g, e->coef, vec_ok, e->qt, e->lay);
                 nctas = (g.nseg + 127) / 128, segs_per_cta = 128, ctas_per_scan = 0;
-                jpeg_huffman_kernel<<<nctas, 128, 0, e->stream>>>(e->coef, g, e->slots, e->sizes, e->offsets, e->cta_total, e->d_huff);
+                jpeg_huffman_kernel<false><<<nctas, 128, 0, e->stream>>>(e->coef, g, e->slots, e->sizes, e->offsets, e->cta_total, e->d_huff, e->lay);
         }
+        return launch_tail(e, nctas, segs_per_cta, ctas_per_scan, single_pass, two_kernels);
+}
+
+/// the common end of an encode: offset scan + compaction (nothing behind the single-pass form), the copy of the stream size and statistics
+static int launch_tail(ugb200_jpeg_encoder *e, int nctas, int segs_per_cta, int ctas_per_scan, bool single_pass, bool two_kernels)
+{
+        const jpeg_geom &g = e->g;
         if (e->stage_timing) {
                 if (!two_kernels) {
                         cudaEventRecord(e->stage_ev[1], e->stream);
@@ -1918,13 +2133,13 @@ int ugb200_jpeg_encode_device(ugb200_jpeg_encoder *e, const void *src, long pitc
                 cfg.stream = e->stream;
                 cfg.attrs = pdl, cfg.numAttrs = e->stage_timing ? 0 : 1;
                 cfg.gridDim = dim3(1), cfg.blockDim = dim3(1024);
-                cudaLaunchKernelEx(&cfg, jpeg_scan_kernel, e->cta_total, nctas, g, e->total);
+                cudaLaunchKernelEx(&cfg, jpeg_scan_kernel, e->cta_total, nctas, g, e->total, e->lay.nscans);
                 if (e->stage_timing) {
                         cudaEventRecord(e->stage_ev[3], e->stream);
                 }
                 cfg.gridDim = dim3((unsigned) (((long) g.nseg * kCompactLanes + 255) / 256)), cfg.blockDim = dim3(256);
                 cudaLaunchKernelEx(&cfg, jpeg_compact_kernel, (const uint8_t *) e->slots, (const uint32_t *) e->sizes, (const uint32_t *) e->offsets,
-                                   (const uint32_t *) e->cta_total, g, segs_per_cta, ctas_per_scan, e->out, (const uint32_t *) e->total, (uint32_t) e->out_cap);
+                                   (const uint32_t *) e->cta_total, g, segs_per_cta, ctas_per_scan, e->out, (const uint32_t *) e->total, (uint32_t) e->out_cap, e->lay);
         }
         if (e->stage_timing) {
                 if (single_pass) {
@@ -1942,6 +2157,118 @@ int ugb200_jpeg_encode_device(ugb200_jpeg_encoder *e, const void *src, long pitc
         }
         e->pending = true;
         return 0;
+}
+
+void ugb200_jpeg_default_params_ex(struct ugb200_jpeg_params_ex *p)
+{
+        ugb200_jpeg_default_params(&p->base);
+        p->subsampling = 0;
+        p->color_space = UGB200_JPEG_CS_NATIVE;
+}
+
+/// the supported matrix of ugb200_jpeg.h: @returns 0 for the stream of ugb200_jpeg_encode_device (UYVY 4:2:2, RGB 4:4:4), 1 for
+/// FMT_PLANAR with hs x vs luma sampling and pre-processing `prep`, -4 for anything else (chroma upsampling, YCbCr -> RGB, one YCbCr
+/// matrix -> another, subsampled RGB)
+static int resolve_layout(int codec, int sub, int cs, int *hs, int *vs, int *prep)
+{
+        if ((sub != 0 && sub != 444 && sub != 422 && sub != 420) || cs < UGB200_JPEG_CS_NATIVE || cs > UGB200_JPEG_CS_RGB) {
+                return -4;
+        }
+        const bool yuv_cs = cs == UGB200_JPEG_CS_NATIVE || cs == UGB200_JPEG_CS_Y709;  // UYVY and I420 frames are BT.709 YCbCr
+        if (codec == UGB_UYVY && yuv_cs) {
+                if (sub == 0 || sub == 422) {
+                        return 0;
+                }
+                *hs = *vs = 2, *prep = PREP_UYVY;
+                return sub == 420 ? 1 : -4;
+        }
+        if (codec == UGB_I420 && yuv_cs) {
+                *hs = *vs = 2, *prep = PREP_NONE;
+                return sub == 0 || sub == 420 ? 1 : -4;
+        }
+        if (codec == UGB_RGB) {
+                if (cs == UGB200_JPEG_CS_NATIVE || cs == UGB200_JPEG_CS_RGB) {
+                        return sub == 0 || sub == 444 ? 0 : -4;
+                }
+                *hs = sub == 422 || sub == 420 ? 2 : 1, *vs = sub == 420 ? 2 : 1, *prep = PREP_RGB + cs;
+                return 1;
+        }
+        return -4;
+}
+
+/// FMT_PLANAR: pre-processing (unless the I420 frame is read in place), then the split path
+static int encode_planar(ugb200_jpeg_encoder *e, const void *src, long pitch, int width, int height, int codec, const struct ugb200_jpeg_params *params,
+                         int hs, int vs, int prep)
+{
+        if (codec == UGB_I420 && pitch != 0) {
+                return -1;  // I420 is three tight planes (vc_get_datalen)
+        }
+        const bool rgb = codec == UGB_RGB;
+        if (pitch == 0) {
+                pitch = (long) width * (rgb ? 3 : 2);  // as ugb200_jpeg_encode_device
+        }
+        const int ri = params->restart_interval > 0 ? params->restart_interval : rgb ? 8 : 4;  // gpujpeg.cpp:351: by the input format
+        const int interleaved = rgb ? (params->interleaved ? 1 : 0) : 1;                       // gpujpeg.cpp:303: UYVY / I420 one scan
+        int rc = configure(e, FMT_PLANAR, width, height, params->quality, ri, interleaved, hs, vs, prep);
+        if (rc != 0) {
+                return rc;
+        }
+        const jpeg_geom &g = e->g;
+        jpeg_layout &L = e->lay;
+        if (prep == PREP_NONE) {  // UltraGrid's I420 frame: Y w x h, then Cb and Cr of ceil(w / 2) x ceil(h / 2) each, tightly packed
+                const uint8_t *y = (const uint8_t *) src;
+                const size_t cn = (size_t) L.plane_w[1] * L.plane_h[1];
+                L.plane[0] = y, L.plane[1] = y + (size_t) width * height, L.plane[2] = y + (size_t) width * height + cn;
+                L.plane_pitch[0] = width, L.plane_pitch[1] = L.plane_pitch[2] = L.plane_w[1];
+        }
+        if (e->stats_pending && cudaEventQuery(e->stats_ev) == cudaSuccess) {
+                adapt_cap(e);
+        }
+        if (prep != PREP_NONE) {
+                jpeg_prep_args a{};
+                a.src = (const uint8_t *) src, a.pitch = pitch, a.w = width, a.h = height, a.rgb = rgb, a.hs = hs, a.vs = vs;
+                a.cw = L.plane_w[1], a.ch = L.plane_h[1];
+                if (rgb) {
+                        const color_coeffs c = prep == PREP_RGB + UGB200_JPEG_CS_Y709 ? coeffs_709(8) : prep == PREP_RGB + UGB200_JPEG_CS_Y601 ? coeffs_601(8) : coeffs_601(0);
+                        const int k[9] = { c.y_r, c.y_g, c.y_b, c.cb_r, c.cb_g, c.cb_b, c.cr_r, c.cr_g, c.cr_b };
+                        memcpy(a.c, k, sizeof k);
+                        a.off_y = prep == PREP_RGB + UGB200_JPEG_CS_Y601FULL ? 0 : 16;
+                }
+                for (int c = 0; c < 3; ++c) {
+                        a.p[c] = (uint8_t *) L.plane[c], a.pp[c] = L.plane_pitch[c];
+                }
+                const long n = (long) a.cw * a.ch;
+                jpeg_prep_kernel<<<(unsigned) ((n + 255) / 256), 256, 0, e->stream>>>(a);
+        }
+        bool vec_ok = true;  // 8-byte row loads
+        for (int c = 0; c < 3; ++c) {
+                vec_ok = vec_ok && !(7 & (size_t) L.plane[c]) && !(7 & L.plane_pitch[c]);
+        }
+        e->last_src = src, e->last_pitch = pitch, e->last_vec_ok = vec_ok, e->last_fused = false;
+        if (e->stage_timing) {
+                cudaEventRecord(e->stage_ev[0], e->stream);
+        }
+        jpeg_dct_kernel<true><<<(g.nblocks + 127) / 128, 128, 0, e->stream>>>(nullptr, 0, g, e->coef, vec_ok, e->qt, L);
+        const int nctas = (g.nseg + 127) / 128;
+        jpeg_huffman_kernel<true><<<nctas, 128, 0, e->stream>>>(e->coef, g, e->slots, e->sizes, e->offsets, e->cta_total, e->d_huff, L);
+        return launch_tail(e, nctas, 128, 0, false, false);
+}
+
+int ugb200_jpeg_encode_device_ex(ugb200_jpeg_encoder *e, const void *src, long pitch, int width, int height, int codec,
+                                 const struct ugb200_jpeg_params_ex *params)
+{
+        if (!e || !src || width <= 0 || height <= 0 || width > 65535 || height > 65535 || !params) {
+                return -1;
+        }
+        int hs = 1, vs = 1, prep = PREP_NONE;
+        const int layout = resolve_layout(codec, params->subsampling, params->color_space, &hs, &vs, &prep);
+        if (layout < 0) {
+                return layout;
+        }
+        if (layout == 0) {
+                return ugb200_jpeg_encode_device(e, src, pitch, width, height, codec, &params->base);
+        }
+        return encode_planar(e, src, pitch, width, height, codec, &params->base, hs, vs, prep);
 }
 
 int ugb200_jpeg_encoder_stage_timing(ugb200_jpeg_encoder *e, int enable)
@@ -1999,23 +2326,31 @@ int ugb200_jpeg_result_device(ugb200_jpeg_encoder *e, const void **dev_ptr, size
         return 0;
 }
 
-/// shared body of ugb200_jpeg_encode / ugb200_jpeg_encode_into: upload (host source), encode, wait, stream to `dst` (host)
+/// shared body of ugb200_jpeg_encode(_into)(_ex): upload (host source), encode, wait, stream to `dst` (host).  I420 only through the _ex calls
 static int encode_to_host(ugb200_jpeg_encoder *e, const void *src, int src_is_device, long pitch, int width, int height, int codec,
-                          const struct ugb200_jpeg_params *params, uint8_t *dst, size_t dst_cap, uint8_t **out, size_t *out_size)
+                          const struct ugb200_jpeg_params_ex *params, bool ex, uint8_t *dst, size_t dst_cap, uint8_t **out, size_t *out_size)
 {
         if (!e || !src || !out_size || width <= 0 || height <= 0) {
                 return -1;
         }
-        const int bpp = codec == UGB_UYVY ? 2 : codec == UGB_RGB ? 3 : 0;
+        const int bpp = codec == UGB_UYVY ? 2 : codec == UGB_RGB ? 3 : codec == UGB_I420 && ex ? 1 : 0;
         if (bpp == 0) {
                 return -4;
         }
         const void *dsrc = src;
         if (!src_is_device) {
-                if (pitch == 0) {
-                        pitch = (long) width * bpp;
+                size_t n;
+                if (codec == UGB_I420) {  // vc_get_datalen (host/video_codec.cpp:56-58); three tight planes, no pitch
+                        if (pitch != 0) {
+                                return -1;
+                        }
+                        n = (size_t) width * height + 2 * (size_t) ((width + 1) / 2) * ((height + 1) / 2);
+                } else {
+                        if (pitch == 0) {
+                                pitch = (long) width * bpp;
+                        }
+                        n = (size_t) pitch * height;
                 }
-                const size_t n = (size_t) pitch * height;
                 if (!grow(e->staging, e->staging_cap, n)) {
                         return -2;
                 }
@@ -2024,7 +2359,8 @@ static int encode_to_host(ugb200_jpeg_encoder *e, const void *src, int src_is_de
                 }
                 dsrc = e->staging;
         }
-        int rc = ugb200_jpeg_encode_device(e, dsrc, pitch, width, height, codec, params);
+        int rc = ex ? ugb200_jpeg_encode_device_ex(e, dsrc, pitch, width, height, codec, params)
+                    : ugb200_jpeg_encode_device(e, dsrc, pitch, width, height, codec, params ? &params->base : nullptr);
         if (rc != 0) {
                 return rc;
         }
@@ -2058,7 +2394,11 @@ int ugb200_jpeg_encode(ugb200_jpeg_encoder *e, const void *src, int src_is_devic
         if (!out) {
                 return -1;
         }
-        return encode_to_host(e, src, src_is_device, pitch, width, height, codec, params, nullptr, 0, out, out_size);
+        ugb200_jpeg_params_ex px{};
+        if (params) {
+                px.base = *params;
+        }
+        return encode_to_host(e, src, src_is_device, pitch, width, height, codec, params ? &px : nullptr, false, nullptr, 0, out, out_size);
 }
 
 int ugb200_jpeg_encode_into(ugb200_jpeg_encoder *e, const void *src, int src_is_device, long pitch, int width, int height, int codec,
@@ -2067,7 +2407,20 @@ int ugb200_jpeg_encode_into(ugb200_jpeg_encoder *e, const void *src, int src_is_
         if (!dst) {
                 return -1;
         }
-        return encode_to_host(e, src, src_is_device, pitch, width, height, codec, params, dst, dst_cap, nullptr, out_size);
+        ugb200_jpeg_params_ex px{};
+        if (params) {
+                px.base = *params;
+        }
+        return encode_to_host(e, src, src_is_device, pitch, width, height, codec, params ? &px : nullptr, false, dst, dst_cap, nullptr, out_size);
+}
+
+int ugb200_jpeg_encode_into_ex(ugb200_jpeg_encoder *e, const void *src, int src_is_device, long pitch, int width, int height, int codec,
+                               const struct ugb200_jpeg_params_ex *params, uint8_t *dst, size_t dst_cap, size_t *out_size)
+{
+        if (!dst) {
+                return -1;
+        }
+        return encode_to_host(e, src, src_is_device, pitch, width, height, codec, params, true, dst, dst_cap, nullptr, out_size);
 }
 
 int ugb200_jpeg_debug_coefficients(ugb200_jpeg_encoder *e, const int16_t **dev_ptr, size_t *count)
@@ -2078,7 +2431,11 @@ int ugb200_jpeg_debug_coefficients(ugb200_jpeg_encoder *e, const int16_t **dev_p
         {  // recompute them with the stand-alone DCT kernel from the last source frame (which must still be alive)
                 const jpeg_geom &g = e->g;
                 const int dct_ctas = g.fmt == FMT_UYVY_422 ? (g.mcu_per_scan + 31) / 32 : (g.nblocks + 127) / 128;
-                jpeg_dct_kernel<<<dct_ctas, 128, 0, e->stream>>>((const uint8_t *) e->last_src, e->last_pitch, g, e->coef, e->last_vec_ok, e->qt);
+                if (g.fmt == FMT_PLANAR) {  // the planes of the last encode (I420: its source frame)
+                        jpeg_dct_kernel<true><<<dct_ctas, 128, 0, e->stream>>>(nullptr, 0, g, e->coef, e->last_vec_ok, e->qt, e->lay);
+                } else {
+                        jpeg_dct_kernel<false><<<dct_ctas, 128, 0, e->stream>>>((const uint8_t *) e->last_src, e->last_pitch, g, e->coef, e->last_vec_ok, e->qt, e->lay);
+                }
         }
         cudaStreamSynchronize(e->stream);
         *dev_ptr = e->coef;

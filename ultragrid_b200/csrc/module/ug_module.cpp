@@ -272,12 +272,12 @@ shared_ptr<video_frame> jpeg_worker::compress_step(shared_ptr<video_frame> tx)  
         const struct video_desc desc = video_desc_from_frame(tx.get());
         const unsigned w = desc.width, h = desc.height;
         if (!video_desc_eq(desc, saved_desc)) {  // configure_with, :256-369
-                enc_input_codec = pick_input_codec(desc.color_spec, { UYVY, RGB });
+                enc_input_codec = desc.color_spec == I420 ? I420 : pick_input_codec(desc.color_spec, { UYVY, RGB });  // I420 as it is (gpujpeg.cpp:262-266)
                 if (enc_input_codec == VIDEO_CODEC_NONE) {
                         fprintf(stderr, "[GPUJPEG] Unsupported codec: %s\n", get_codec_name(desc.color_spec));
                         return {};
                 }
-                if (!parent->opts.check_against_input(enc_input_codec == RGB)) {
+                if (!parent->opts.check_against_input(enc_input_codec == RGB ? jpeg_input::RGB : enc_input_codec == I420 ? jpeg_input::I420 : jpeg_input::UYVY)) {
                         return {};
                 }
                 struct video_desc compressed = desc;
@@ -302,16 +302,18 @@ shared_ptr<video_frame> jpeg_worker::compress_step(shared_ptr<video_frame> tx)  
                 }
                 in = cuda_conv;
         }
-        struct ugb200_jpeg_params p;
-        ugb200_jpeg_default_params(&p);
+        struct ugb200_jpeg_params_ex p;
+        ugb200_jpeg_default_params_ex(&p);
         if (parent->opts.quality != -1) {
-                p.quality = parent->opts.quality;
+                p.base.quality = parent->opts.quality;
         }
-        p.restart_interval = parent->opts.restart_interval;
-        p.interleaved = parent->opts.interleaved ? 1 : 0;
+        p.base.restart_interval = parent->opts.restart_interval;
+        p.base.interleaved = parent->opts.interleaved ? 1 : 0;
+        p.subsampling = parent->opts.subsampling;  // as checked against the input: the input's own layout
+        p.color_space = parent->opts.internal_cs;
         shared_ptr<video_frame> out = pool.get_frame();
         size_t size = 0;
-        if (!out || ugb200_jpeg_encode_into(encoder, in, 1, 0, (int) w, (int) h, (int) enc_input_codec, &p, (uint8_t *) out->tiles[0].data, (size_t) w * h * 3 + 4096, &size) != 0) {
+        if (!out || ugb200_jpeg_encode_into_ex(encoder, in, 1, 0, (int) w, (int) h, (int) enc_input_codec, &p, (uint8_t *) out->tiles[0].data, (size_t) w * h * 3 + 4096, &size) != 0) {
                 return {};
         }
         out->tiles[0].data_len = (unsigned) size;
