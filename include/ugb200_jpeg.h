@@ -13,8 +13,16 @@
  *   UGB_RGB  input, Y709 | Y601 | Y601FULL   -> YCbCr 4:4:4 / 4:2:2 / 4:2:0 (subsampling 0 = 444), one scan per component (T.81 A.2: a
  *                                               component's blocks are not padded to whole MCUs) or one interleaved scan with `interleaved`;
  *                                               integer RGB_TO_Y/CB/CR of the reference at 8 bits (Y601FULL: JFIF full range)
- *   every YCbCr stream carries JFIF APP0; restart interval default 8 for RGB input, 4 otherwise.  Native parameters give the bytes of
- *   the calls without _ex.  Anything else returns -4: chroma upsampling, YCbCr -> RGB, one YCbCr matrix -> another, subsampled RGB.
+ *   UGB_RGBA input, subsampling 4444, colour space NATIVE or RGB (the GPUJPEG module's `alpha`: GPUJPEG_SUBSAMPLING_4444 with
+ *                                               GPUJPEG_4444_U8_P0123, gpujpeg.cpp:227-236,316-328) -> R, G, B, A stored as-is, the frame read in
+ *                                               place at 4 B/px: Adobe APP14 transform 0, SOF0 with four components (ids 1..4, all 1x1,
+ *                                               quantisation and Huffman tables 0 1 1 1 - GPUJPEG's own choice for alpha is unpinned, the library
+ *                                               being absent), four scans (one per component, gpujpeg.cpp:303) or one scan of R G B A MCUs with
+ *                                               `interleaved`, restart interval default 8.  The first three scans are byte for byte the scans of
+ *                                               the RGB stream of the frame's R, G, B bytes; the fourth is coded like the third (table 1).
+ *   every YCbCr stream carries JFIF APP0; restart interval default 8 for RGB and RGBA input, 4 otherwise.  Native parameters give the bytes
+ *   of the calls without _ex.  Anything else returns -4: chroma upsampling, YCbCr -> RGB, one YCbCr matrix -> another, subsampled RGB, RGBA
+ *   without subsampling 4444 or with a YCbCr colour space, and RGBA through ugb200_jpeg_encode_device / _encode / _encode_into.
  * Output capacity is width*height*3 + 4096 bytes like the reference's pool frames (gpujpeg.cpp:355).
  */
 #ifndef UGB200_JPEG_H
@@ -59,7 +67,7 @@ struct ugb200_jpeg_params_ex {
         int color_space;   /* UGB200_JPEG_CS_* */
 };
 UGB_API void ugb200_jpeg_default_params_ex(struct ugb200_jpeg_params_ex *p);
-/* ugb200_jpeg_encode_device with the layouts above; `codec` also takes UGB_I420 (pitch must be 0) */
+/* ugb200_jpeg_encode_device with the layouts above; `codec` also takes UGB_I420 (pitch must be 0) and UGB_RGBA (subsampling 4444) */
 UGB_API int ugb200_jpeg_encode_device_ex(ugb200_jpeg_encoder *enc, const void *src, long pitch, int width, int height, int codec,
                                          const struct ugb200_jpeg_params_ex *params);
 
@@ -95,7 +103,11 @@ UGB_API int ugb200_jpeg_debug_coefficients(ugb200_jpeg_encoder *enc, const int16
  * Baseline sequential Huffman JPEG, 3 components, luma sampling 1x1 / 2x1 / 2x2, interleaved or one scan per component, restart
  * intervals (the unit of GPU parallelism), tables taken from the stream.  No colour transform inside the codec: a 4:2:2 / 4:2:0
  * YCbCr stream decodes to UYVY, a 4:4:4 RGB stream (Adobe transform 0) to RGB, a 4:4:4 YCbCr stream to VUYA; any other requested
- * output goes through UltraGrid's own line converters (ugb200_pixfmt_convert). */
+ * output goes through UltraGrid's own line converters (ugb200_pixfmt_convert).
+ * Also 4 components, all sampled 1x1, without an Adobe marker or with Adobe transform 0 (the GPUJPEG module's `alpha` stream): native
+ * codec UGB_RGBA, samples as stored.  To RGBA with shifts (0, 8, 16): R G B A, alpha in byte 3, at any pitch; with other shifts that
+ * result re-shifted by the RGBA -> RGBA line converter (vc_copylineRGBA: the unused byte becomes 0xFF).  To any other codec: the first three
+ * planes as an RGB stream decodes.  Four-component streams with Adobe transform 1 or 2 (YCCK) or subsampled components return -4. */
 typedef struct ugb200_jpeg_decoder ugb200_jpeg_decoder;
 struct ugb200_jpeg_image_info {
         int width, height, components;

@@ -60,6 +60,15 @@ for codec, sub, cs, il in ([] if ONLY == "staged" else ((29, 0, 0, 1), (2, 420, 
         if sub == 420 or codec == 29:
             dec.decode(s, 29)
         n += 2
+# JPEG with alpha: RGBA 4444 on tight buffers, four scans (fused kernel; restart interval 5: split path) and one interleaved scan (split path);
+# the four-component streams decode to RGBA, RGB and UYVY
+for w, h, ri, il in ([] if ONLY == "staged" else ((17, 9, 0, 0), (130, 37, 5, 0), (130, 37, 0, 1))):
+    src = torch.randint(0, 256, (w * h * 4,), dtype=torch.uint8, device="cuda")
+    enc.encode_device(src, w, h, 1, quality=90, restart_interval=ri, interleaved=bool(il), subsampling=4444)
+    s = enc.result()
+    for out_c in (1, 12, 2):
+        dec.decode(s, out_c)
+    n += 4
 # round 2, state i: the staged launch forms of the line converters (16-byte aligned pitches, tight buffers), every form of every converter
 for inc, outc in ([] if ONLY == "jpeg" else PAIRS):
     for w, h in ((64, 2), (192, 3), (2048 + 64, 2)):

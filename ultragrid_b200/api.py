@@ -218,7 +218,8 @@ class JpegParams(ctypes.Structure):
 
 
 class JpegParamsEx(ctypes.Structure):
-    """struct ugb200_jpeg_params_ex: subsampling 0 (native) / 444 / 422 / 420, color_space one of JPEG_CS"""
+    """struct ugb200_jpeg_params_ex: subsampling 0 (native) / 444 / 422 / 420, or 4444 with Codec.RGBA (R G B A, the alpha channel
+    as a fourth component); color_space one of JPEG_CS"""
     _fields_ = [("base", JpegParams), ("subsampling", ctypes.c_int), ("color_space", ctypes.c_int)]
 
 

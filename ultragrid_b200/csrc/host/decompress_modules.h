@@ -68,8 +68,8 @@ static decompress_status gpujpeg_probe_internal_codec(unsigned char *buffer, siz
                 return DECODER_NO_FRAME;
         }
         internal_prop->depth = 8;
-        internal_prop->rgb = info.native_codec == RGB;
-        internal_prop->subsampling = info.h_samp == 1 ? SUBS_444 : info.v_samp == 1 ? SUBS_422 : SUBS_420;
+        internal_prop->rgb = info.native_codec == RGB || info.native_codec == RGBA;  // four components: R G B A (gpujpeg.c:254-260)
+        internal_prop->subsampling = info.components == 4 ? SUBS_4444 : info.h_samp == 1 ? SUBS_444 : info.v_samp == 1 ? SUBS_422 : SUBS_420;
         return DECODER_GOT_CODEC;
 }
 static decompress_status gpujpeg_decompress(void *state, unsigned char *dst, unsigned char *buffer, unsigned int src_len, int, struct video_frame_callbacks *,

@@ -4,7 +4,8 @@
 //     <quality>[:<restart interval>] positionally, or quality=<n> (here also q=<n>), restart=<n>, interleaved, Y601 | Y601full | Y709 | RGB,
 //     subsampling=<444|422|420>, alpha; plus lanes=<n> (addition of this library: frames in flight per device).
 // This module stores the input as it comes (RGB input -> RGB, 4:4:4; UYVY input -> BT.709 YCbCr, 4:2:2; I420 input -> BT.709 YCbCr, 4:2:0 - the
-// reference's own defaults, :295-305, :332): an internal colour space or a subsampling other than the input's own is refused when the first frame
+// reference's own defaults, :295-305, :332; RGBA input with `alpha` -> R G B A, four components 1x1, :227-236,316-328): an internal colour space or a
+// subsampling other than the input's own is refused when the first frame
 // shows the input format (check_against_input), with a message instead of a silently different stream.  The encoder itself can also convert
 // RGB to YCbCr and subsample chroma (ugb200_jpeg_encode_into_ex); opening those options here is a change of this policy only.
 #pragma once
@@ -15,7 +16,7 @@
 #include <string>
 #include <strings.h>
 
-enum class jpeg_input { UYVY, RGB, I420 };  // the encoder input formats
+enum class jpeg_input { UYVY, RGB, I420, RGBA };  // the encoder input formats (RGBA: only with `alpha`, read in place)
 
 struct gpujpeg_opts {
         int quality = -1;           // -1: encoder default (gpujpeg_set_default_parameters: 75)
@@ -23,7 +24,7 @@ struct gpujpeg_opts {
         bool interleaved = false;   // m_force_interleaved
         int internal_cs = 0;        // 0 unset, 1 Y601, 2 Y601full, 3 Y709, 4 RGB
         int subsampling = 0;        // 0 auto, else 444 / 422 / 420
-        bool alpha = false;
+        bool alpha = false;         // RGBA input: four components (the alpha channel kept)
         int lanes = 3;
         bool help = false;
 
@@ -103,16 +104,28 @@ struct gpujpeg_opts {
 
         static void usage()
         {
-                printf("GPUJPEG usage:\n\t-c GPUJPEG[:<quality>[:<restart_interval>]][:quality=<q>][:restart=<n>][:interleaved][:RGB|Y709][:subsampling=<444|422|420>][:lanes=<n>]\n"
-                       "\twhere\n\t\tinterleaved - one scan for RGB input too (default: one scan per component)\n"
+                printf("GPUJPEG usage:\n\t-c GPUJPEG[:<quality>[:<restart_interval>]][:quality=<q>][:restart=<n>][:interleaved][:RGB|Y709][:subsampling=<444|422|420>][:alpha][:lanes=<n>]\n"
+                       "\twhere\n\t\tinterleaved - one scan for RGB and RGBA input too (default: one scan per component)\n"
                        "\t\tRGB|Y709 - must name the colour space the input already has (no transform inside the codec)\n"
                        "\t\tsubsampling - must name the input's own: 444 for RGB, 422 for UYVY, 420 for I420 (I420 frames are encoded as they are)\n"
+                       "\t\talpha - RGBA input is encoded with its alpha channel as a fourth component (subsampling 4:4:4:4; RGB colour space only)\n"
                        "\t\tlanes - frames in flight per CUDA device (default 3)\n");
         }
 
         /// the options against the encoder input format: what needs a transform inside the codec is refused
         bool check_against_input(jpeg_input in) const
         {
+                if (in == jpeg_input::RGBA) {  // `alpha` with RGBA frames: R G B A as stored, every component 1x1
+                        if (internal_cs != 0 && internal_cs != 4) {
+                                fprintf(stderr, "[GPUJPEG] alpha: RGBA input is stored as R G B A; the requested internal colour space needs a colour transform inside the codec\n");
+                                return false;
+                        }
+                        if (subsampling != 0 && subsampling != 444) {
+                                fprintf(stderr, "[GPUJPEG] alpha: subsampling=%d needs resampling inside the codec; RGBA input is stored as 4:4:4:4\n", subsampling);
+                                return false;
+                        }
+                        return true;
+                }
                 const char *name = in == jpeg_input::RGB ? "RGB" : in == jpeg_input::UYVY ? "UYVY" : "I420";
                 if (internal_cs != 0 && internal_cs != (in == jpeg_input::RGB ? 4 : 3)) {
                         fprintf(stderr, "[GPUJPEG] the requested internal colour space needs a colour transform inside the codec; this encoder stores %s input as %s\n",
@@ -126,7 +139,7 @@ struct gpujpeg_opts {
                         return false;
                 }
                 if (alpha) {
-                        fprintf(stderr, "[GPUJPEG] Requested alpha encode but the encoder stores three components; alpha is dropped\n");
+                        fprintf(stderr, "[GPUJPEG] Requested alpha encode but the input is not RGBA; alpha is dropped\n");
                 }
                 return true;
         }

@@ -487,11 +487,16 @@ std::shared_ptr<video_frame> encoder_state::compress_step(std::shared_ptr<video_
                 const codec_t supported[] = { UYVY, RGB, VIDEO_CODEC_NONE };
                 if (desc.color_spec == I420) {  // planar I420 goes into the encoder as it is (gpujpeg.cpp:262-266)
                         enc_input_codec = I420;
+                } else if (desc.color_spec == RGBA && parent->opts.alpha) {  // RGBA with `alpha`: read in place, four components (:227-236)
+                        enc_input_codec = RGBA;
                 } else if (!get_best_decoder_from(desc.color_spec, supported, &enc_input_codec)) {
                         fprintf(stderr, "[GPUJPEG] Unsupported codec: %s\n", get_codec_name(desc.color_spec));
                         return {};
                 }
-                if (!parent->opts.check_against_input(enc_input_codec == RGB ? jpeg_input::RGB : enc_input_codec == I420 ? jpeg_input::I420 : jpeg_input::UYVY)) {
+                if (!parent->opts.check_against_input(enc_input_codec == RGB    ? jpeg_input::RGB
+                                                      : enc_input_codec == I420 ? jpeg_input::I420
+                                                      : enc_input_codec == RGBA ? jpeg_input::RGBA
+                                                                                : jpeg_input::UYVY)) {
                         return {};
                 }
                 saved_desc = desc;
@@ -543,6 +548,9 @@ std::shared_ptr<video_frame> encoder_state::compress_step(std::shared_ptr<video_
         p.base.interleaved = parent->opts.interleaved ? 1 : 0;
         p.subsampling = parent->opts.subsampling;  // as checked against the input: the input's own layout
         p.color_space = parent->opts.internal_cs;
+        if (enc_input_codec == RGBA) {
+                p.subsampling = 4444;  // GPUJPEG_SUBSAMPLING_4444, :316-328
+        }
         // the stream goes straight into the pooled (pinned) output frame: no encoder-owned buffer + memcpy as at :629-630
         const size_t out_cap = (size_t) w * h * 3 + 4096;  // :355 plus the header allowance of the encoder's own buffer (ugb200_jpeg.h): tiny or
                                                            // noisy frames at high quality exceed the raw size by their ~600-byte header

@@ -61,14 +61,14 @@ struct dec_comp {
         long plane_off; // first byte of the plane in the plane buffer
 };
 struct dec_scan {
-        int ns, comp[3], td[3], ta[3];
+        int ns, comp[4], td[4], ta[4];
         int mcux, nmcu;
         int seg0, nseg;  // segments [seg0, seg0 + nseg)
 };
 struct dec_geom {
-        int w, h, ncomp, hmax, vmax, ri, nscans, nblocks;
-        dec_comp c[3];
-        dec_scan s[3];
+        int w, h, ncomp, hmax, vmax, ri, nscans, nblocks;  // ncomp 3, or 4 (R G B A, all 1x1)
+        dec_comp c[4];
+        dec_scan s[4];
 };
 
 struct bit_reader {  // MSB-first, removes stuffed zero bytes, feeds zeros beyond `end`
@@ -177,7 +177,7 @@ __global__ void __launch_bounds__(kHuffThreads) jpeg_decode_huffman_kernel(const
         const int m0 = g.ri ? ls * g.ri : 0, m1 = g.ri ? min(m0 + g.ri, S.nmcu) : S.nmcu;
         bit_reader r = { stream + seg_begin[s], stream + seg_end[s], 0, 0, nullptr, 0, 0 };
         r.prime();
-        int pred[3] = { 0, 0, 0 };
+        int pred[4] = { 0, 0, 0, 0 };
         for (int m = m0; m < m1; ++m) {
                 const int mx = m % S.mcux, my = m / S.mcux;
                 for (int k = 0; k < S.ns; ++k) {
@@ -709,7 +709,7 @@ constexpr long kMaxPixels = 16384L * 16384L;  // four 8K frames side by side; la
 
 struct parsed {
         dec_geom g{};
-        int adobe = -1, comp_id[3] = { 0, 0, 0 };
+        int adobe = -1, comp_id[4] = { 0, 0, 0, 0 };
         bool have_sof = false, have_q[4] = { false, false, false, false };
         uint8_t q[4][64];
         std::vector<uint32_t> seg_begin, seg_end;
@@ -880,23 +880,23 @@ int parse_stream(const uint8_t *s, size_t len, parsed &P, dec_tables *T, bool fu
                                 return -4;
                         }
                         g.h = be16(d + 1), g.w = be16(d + 3), g.ncomp = d[5];
-                        if (g.ncomp != 3 || g.w == 0 || g.h == 0) {
+                        if ((g.ncomp != 3 && g.ncomp != 4) || g.w == 0 || g.h == 0) {
                                 return -4;
                         }
                         if ((long) g.w * g.h > kMaxPixels) {  // header fields are untrusted: they size every host and device allocation below
                                 return -4;
                         }
                         g.hmax = g.vmax = 1;
-                        for (int i = 0; i < 3; ++i) {
+                        for (int i = 0; i < g.ncomp; ++i) {
                                 P.comp_id[i] = d[6 + 3 * i];
                                 g.c[i].h = d[7 + 3 * i] >> 4, g.c[i].v = d[7 + 3 * i] & 15, g.c[i].tq = d[8 + 3 * i];
                                 g.hmax = g.c[i].h > g.hmax ? g.c[i].h : g.hmax, g.vmax = g.c[i].v > g.vmax ? g.c[i].v : g.vmax;
                         }
                         int blk = 0;
                         long off = 0;
-                        for (int i = 0; i < 3; ++i) {
+                        for (int i = 0; i < g.ncomp; ++i) {  // four components: every one sampled 1x1 (no subsampled alpha)
                                 dec_comp &c = g.c[i];
-                                if (c.h < 1 || c.h > 2 || c.v < 1 || c.v > 2 || (i > 0 && (c.h != 1 || c.v != 1)) || c.tq > 3) {
+                                if (c.h < 1 || c.h > 2 || c.v < 1 || c.v > 2 || ((i > 0 || g.ncomp == 4) && (c.h != 1 || c.v != 1)) || c.tq > 3) {
                                         return -4;
                                 }
                                 c.bw = (g.w + 8 * g.hmax - 1) / (8 * g.hmax) * c.h, c.bh = (g.h + 8 * g.vmax - 1) / (8 * g.vmax) * c.v;
@@ -915,20 +915,23 @@ int parse_stream(const uint8_t *s, size_t len, parsed &P, dec_tables *T, bool fu
                 } else if (mk == 0xEE && L >= 14 && memcmp(d, "Adobe", 5) == 0) {
                         P.adobe = d[11];
                 } else if (mk == 0xDA) {
-                        if (!P.have_sof || g.nscans >= 3) {
+                        if (!P.have_sof || g.nscans >= g.ncomp) {
                                 return -3;
+                        }
+                        if (g.ncomp == 4 && P.adobe != -1 && P.adobe != 0) {
+                                return -4;  // Adobe transform 2 (YCCK) or 1: samples are not R G B A as stored
                         }
                         dec_scan &S = g.s[g.nscans];
                         if (L < 3) {
                                 return -3;
                         }
                         S.ns = d[0];
-                        if (S.ns < 1 || S.ns > 3 || L < 6 + 2 * S.ns) {
+                        if (S.ns < 1 || S.ns > g.ncomp || L < 6 + 2 * S.ns) {
                                 return -4;
                         }
                         for (int i = 0; i < S.ns; ++i) {
                                 S.comp[i] = -1;
-                                for (int j = 0; j < 3; ++j) {
+                                for (int j = 0; j < g.ncomp; ++j) {
                                         if (P.comp_id[j] == d[1 + 2 * i]) {
                                                 S.comp[i] = j;
                                         }
@@ -1024,6 +1027,9 @@ void collect_markers(const uint8_t *stream, size_t len, scan_pool *pool, uint8_t
 int native_codec(const parsed &P)
 {
         const dec_geom &g = P.g;
+        if (g.ncomp == 4) {
+                return UGB_RGBA;  // R G B A as stored (the parser refuses subsampled and YCCK four-component streams)
+        }
         if (g.c[0].h == 2) {
                 return UGB_UYVY;  // 4:2:2 and 4:2:0 land in UYVY
         }
@@ -1287,7 +1293,13 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
         const size_t nseg = multi ? (size_t) (g.s[2].seg0 + g.s[2].nseg) : device_scan ? (size_t) g.s[0].nseg : P.seg_begin.size();
         d->last_nseg = nseg;
         const long plane_bytes = (long) g.nblocks * 64;
-        const int native = native_codec(P);
+        // Four components (R G B A): packed to RGBA when RGBA is asked for - with other shifts than (0, 8, 16) the packed frame then goes through the
+        // RGBA -> RGBA line converter, as vc_copylineRGBA re-shifts it (alpha becomes 0xFF) - and to RGB (the first three planes) for any other
+        // output, which then takes the routes of an RGB stream
+        const int stream_codec = native_codec(P);
+        const bool alpha = stream_codec == UGB_RGBA;
+        const bool reshift = alpha && out_codec == UGB_RGBA && !(rshift == 0 && gshift == 8 && bshift == 16);
+        const int native = alpha && out_codec != UGB_RGBA ? UGB_RGB : stream_codec;
         const long npitch = native == UGB_UYVY ? (long) ((g.w + 1) / 2) * 4 : native == UGB_RGB ? (long) g.w * 3 : (long) g.w * 4;
         const long opitch = out_codec == UGB_UYVY ? (long) ((g.w + 1) / 2) * 4 : out_codec == UGB_RGB ? (long) g.w * 3 : (long) g.w * 4;
         if (dst_pitch == 0) {
@@ -1353,7 +1365,7 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
         // truncated multi-scan stream - is covered by nobody.)  Then the Huffman kernel writes whole blocks and the array is not cleared.
         bool full = true;
         {
-                int seen[3] = { 0, 0, 0 };
+                int seen[4] = { 0, 0, 0, 0 };
                 for (int j = 0; j < g.nscans; ++j) {
                         const dec_scan &S = g.s[j];
                         for (int k = 0; k < S.ns; ++k) {
@@ -1364,7 +1376,7 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
                                 full = full && S.mcux == c.bw && S.nmcu == c.bw * c.bh;
                         }
                 }
-                full = full && seen[0] == 1 && seen[1] == 1 && seen[2] == 1;
+                full = full && seen[0] == 1 && seen[1] == 1 && seen[2] == 1 && (g.ncomp == 3 || seen[3] == 1);
         }
         const unsigned hgrid = (unsigned) ((nseg + kHuffThreads - 1) / kHuffThreads);
         const size_t hsmem = ((sizeof(dec_tables) + 15) & ~(size_t) 15) + (size_t) kHuffThreads * 128;
@@ -1377,7 +1389,7 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
         }
         cudaEventRecord(H.consumed, s);  // nothing behind this kernel reads the stream
         H.consumed_pending = true;
-        const bool direct = native == out_codec && dst_is_device;
+        const bool direct = native == out_codec && dst_is_device && !reshift;
         uint8_t *nat = direct ? (uint8_t *) dst : d->native;
         const bool fused_uyvy = native == UGB_UYVY && g.c[0].v == 1;  // 4:2:2: IDCT and packing in one kernel, no component planes
         if (fused_uyvy) {
@@ -1400,8 +1412,16 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
                 fp.in_data[i] = d->planes + g.c[i].plane_off, fp.in_linesize[i] = (unsigned) (g.c[i].bw * 8);
         }
         fp.in_depth = 8;
+        if (alpha) {  // planes in G, B, R, A order (from_planar.c:335-366); all four have the same line size
+                for (int i = 0; i < 4; ++i) {
+                        const dec_comp &c = g.c[i == 3 ? 3 : (i + 1) % 3];
+                        fp.in_data[i] = d->planes + c.plane_off, fp.in_linesize[i] = (unsigned) (c.bw * 8);
+                }
+        }
         if (fused_uyvy) {
                 rc = 0;
+        } else if (alpha) {
+                rc = native == UGB_RGBA ? ugb200_gbrap_to_rgba(&fp, s) : ugb200_gbrap_to_rgb(&fp, s);
         } else if (native == UGB_UYVY) {
                 rc = g.c[0].v == 2 ? ugb200_yuv420p_to_uyvy(&fp, s) : ugb200_yuv422p_to_uyvy(&fp, s);
         } else if (native == UGB_RGB) {
@@ -1449,7 +1469,7 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
         // native -> requested codec (UltraGrid's own line converters), then to the caller
         uint8_t *result = nat;
         long rpitch = npitch;
-        if (native != out_codec) {
+        if (native != out_codec || reshift) {
                 if (!ugb200_pixfmt_supported(native, out_codec)) {
                         return -4;
                 }
