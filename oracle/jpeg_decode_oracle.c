@@ -292,7 +292,7 @@ API int orc_jpeg_decode(const uint8_t *s, size_t len, int out_fmt, uint8_t *out,
                         }
                         for (int i = 0; i < f.ncomp; ++i) {
                                 struct comp *c = &f.c[i];
-                                if (c->h < 1 || c->h > 2 || c->v < 1 || c->v > 2 || (i > 0 && (c->h != 1 || c->v != 1))) {
+                                if (c->h < 1 || c->h > 2 || c->v < 1 || c->v > 2 || (i > 0 && (c->h != 1 || c->v != 1)) || c->v > c->h) { /* no luma 1x2 */
                                         rc = -4;
                                         break;
                                 }

@@ -44,12 +44,17 @@ static const uint8_t kZigzag[64] = { 0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32,
                                      30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63 };
 
 constexpr int kLook = 9;
+/// Huffman table slots.  A DHT definition is built into a slot when a scan first uses it: table id k (DC Th 0, 1 = 0, 1; AC Th 0, 1 = 2, 3)
+/// goes to slot k when that slot is free, otherwise to the lowest free one.  A table redefined between scans (T.81 B.2.4.2) thus gets a slot
+/// of its own, and every scan keeps the tables it was coded with.  In a valid stream each component appears in one scan and uses one DC and
+/// one AC table, and only definitions that a scan uses take a slot: four components never need more than eight.
+constexpr int kTables = 8;
 
-struct dec_tables {                   // tables 0,1 = DC (Th 0,1), 2,3 = AC (Th 0,1)
-        uint16_t lut[4][1 << kLook];  // (length << 8) | symbol for codes of up to kLook bits, 0 = longer code
-        int maxcode[4][18];           // T.81 F.2.2.3, -1 = no code of that length
-        int valoff[4][17];            // valptr - mincode
-        uint8_t vals[4][256];
+struct dec_tables {
+        uint16_t lut[kTables][1 << kLook];  // (length << 8) | symbol for codes of up to kLook bits, 0 = longer code
+        int maxcode[kTables][18];           // T.81 F.2.2.3, -1 = no code of that length
+        int valoff[kTables][17];            // valptr - mincode
+        uint8_t vals[kTables][256];
         uint8_t zz[64];
         float m[4][64];               // dequantisation x AAN scale, natural order
 };
@@ -61,12 +66,13 @@ struct dec_comp {
         long plane_off; // first byte of the plane in the plane buffer
 };
 struct dec_scan {
-        int ns, comp[4], td[4], ta[4];
+        int ns, comp[4], td[4], ta[4];  // td, ta: table slots of dec_tables
         int mcux, nmcu;
         int seg0, nseg;  // segments [seg0, seg0 + nseg)
 };
 struct dec_geom {
         int w, h, ncomp, hmax, vmax, ri, nscans, nblocks;  // ncomp 3, or 4 (R G B A, all 1x1)
+        int ntables;  // Huffman table slots in use: [0, ntables) (the Huffman kernel copies only those to shared memory)
         dec_comp c[4];
         dec_scan s[4];
 };
@@ -149,6 +155,14 @@ __device__ __forceinline__ int receive_extend(bit_reader &r, int n)  // F.2.2.1,
 /// kHuffThreads: an 8K UYVY frame has 64 800 restart segments = threads, all resident at once; with 128-thread CTAs that is 3.4 CTAs per SM (some SMs run four, the
 /// kernel lasts as long as those), with 64-thread CTAs 6.8 (seven against six)
 constexpr int kHuffThreads = 64;
+/// block-wide copy of `bytes` (a multiple of 4) between 4-byte aligned addresses
+__device__ __forceinline__ void copy_words(void *dst, const void *src, int bytes)
+{
+        for (int i = threadIdx.x; i < bytes / 4; i += blockDim.x) {
+                ((uint32_t *) dst)[i] = ((const uint32_t *) src)[i];
+        }
+}
+
 template <bool FULL>
 __global__ void __launch_bounds__(kHuffThreads) jpeg_decode_huffman_kernel(const uint8_t *__restrict__ stream, const uint32_t *__restrict__ seg_begin,
                                                                   const uint32_t *__restrict__ seg_end, const dec_tables *__restrict__ tables,
@@ -157,9 +171,12 @@ __global__ void __launch_bounds__(kHuffThreads) jpeg_decode_huffman_kernel(const
         extern __shared__ uint8_t smem_raw[];
         dec_tables *t = (dec_tables *) smem_raw;
         uint32_t *const col = (uint32_t *) (smem_raw + ((sizeof(dec_tables) + 15) & ~(size_t) 15)) + threadIdx.x;  // FULL: word w of my block at col[w * kHuffThreads]
-        for (int i = threadIdx.x; i < (int) (sizeof(dec_tables) / 4); i += blockDim.x) {
-                ((uint32_t *) t)[i] = ((const uint32_t *) tables)[i];
-        }
+        // what this kernel reads: the slots in use and the zig-zag order (not the dequantisation multipliers)
+        copy_words(t->lut, tables->lut, g.ntables * (int) sizeof t->lut[0]);
+        copy_words(t->maxcode, tables->maxcode, g.ntables * (int) sizeof t->maxcode[0]);
+        copy_words(t->valoff, tables->valoff, g.ntables * (int) sizeof t->valoff[0]);
+        copy_words(t->vals, tables->vals, g.ntables * (int) sizeof t->vals[0]);
+        copy_words(t->zz, tables->zz, (int) sizeof t->zz);
         __syncthreads();
         const int s = blockIdx.x * blockDim.x + threadIdx.x;
         int sc = 0;
@@ -171,7 +188,7 @@ __global__ void __launch_bounds__(kHuffThreads) jpeg_decode_huffman_kernel(const
         }
         dec_scan S = g.s[sc];
         if (dev_scans != nullptr && sc > 0) {  // multi-scan stream with the marker scan on the device: the SOS headers of the later scans were read there
-                S.td[0] = (int) dev_scans[kMetaBounds + 6 * sc + 4], S.ta[0] = (int) dev_scans[kMetaBounds + 6 * sc + 5];
+                S.td[0] = (int) dev_scans[kMetaBounds + 6 * sc + 4], S.ta[0] = 2 + (int) dev_scans[kMetaBounds + 6 * sc + 5];  // no DHT between the scans
         }
         const int ls = s - S.seg0;
         const int m0 = g.ri ? ls * g.ri : 0, m1 = g.ri ? min(m0 + g.ri, S.nmcu) : S.nmcu;
@@ -207,7 +224,7 @@ __global__ void __launch_bounds__(kHuffThreads) jpeg_decode_huffman_kernel(const
                                         }
                                         for (int i = 1; i < 64;) {
                                                 r.refill();
-                                                const int rs = decode_symbol(r, t, 2 + S.ta[k]), run = rs >> 4, sz = rs & 15;
+                                                const int rs = decode_symbol(r, t, S.ta[k]), run = rs >> 4, sz = rs & 15;
                                                 if (sz == 0) {
                                                         if (run != 15) {
                                                                 break;  // EOB
@@ -707,17 +724,26 @@ int be16(const uint8_t *p) { return p[0] << 8 | p[1]; }
 
 constexpr long kMaxPixels = 16384L * 16384L;  // four 8K frames side by side; larger SOF dimensions are refused before anything is allocated
 
+struct huff_defs {  // the current DHT definition of each table id, built into a slot of dec_tables when a scan first uses it
+        uint8_t bits[4][16], vals[4][256];
+        int n[4] = { 0, 0, 0, 0 };
+        bool defined[4] = { false, false, false, false };
+        int slot[4] = { -1, -1, -1, -1 };  // slot holding the current definition, -1 = not built yet
+        bool taken[kTables] = {};          // built: a scan reads it
+};
+
 struct parsed {
         dec_geom g{};
         int adobe = -1, comp_id[4] = { 0, 0, 0, 0 };
         bool have_sof = false, have_q[4] = { false, false, false, false };
+        huff_defs hd;
         uint8_t q[4][64];
         std::vector<uint32_t> seg_begin, seg_end;
 };
 
 /// @returns false for an over-subscribed code-length histogram (the Kraft check behind libjpeg's JERR_BAD_HUFF_TABLE): after the codes of
-/// length l are assigned the next code must still fit in l bits, otherwise the look-up fill below would run past the table
-bool build_table(dec_tables &t, int tab, const uint8_t *bits, const uint8_t *vals, int n)
+/// length l are assigned the next code must still fit in l bits, otherwise the look-up fill of build_table would run past the table
+bool kraft_ok(const uint8_t *bits)
 {
         for (int l = 1, code = 0; l <= 16; ++l) {
                 code += bits[l - 1];
@@ -726,6 +752,12 @@ bool build_table(dec_tables &t, int tab, const uint8_t *bits, const uint8_t *val
                 }
                 code <<= 1;
         }
+        return true;
+}
+
+/// the bits / values have passed kraft_ok
+void build_table(dec_tables &t, int tab, const uint8_t *bits, const uint8_t *vals, int n)
+{
         memset(t.lut[tab], 0, sizeof t.lut[tab]);
         memcpy(t.vals[tab], vals, n);
         int code = 0, k = 0;
@@ -742,7 +774,29 @@ bool build_table(dec_tables &t, int tab, const uint8_t *bits, const uint8_t *val
                 code <<= 1;
         }
         t.maxcode[tab][17] = 0x7fffffff;
-        return true;
+}
+
+/// the table slot of the current definition of table id `id`, built on first use (see kTables); -1: the table is undefined or no slot is left
+int table_slot(huff_defs &H, dec_tables *T, int id)
+{
+        if (!H.defined[id]) {
+                return -1;
+        }
+        if (H.slot[id] < 0) {
+                int k = id;
+                if (H.taken[k]) {
+                        for (k = 0; k < kTables && H.taken[k]; ++k) {
+                        }
+                        if (k == kTables) {
+                                return -1;
+                        }
+                }
+                H.taken[k] = true, H.slot[id] = k;
+                if (T) {
+                        build_table(*T, k, H.bits[id], H.vals[id], H.n[id]);
+                }
+        }
+        return H.slot[id];
 }
 
 const bool g_stream_stores = [] {
@@ -870,9 +924,12 @@ int parse_stream(const uint8_t *s, size_t len, parsed &P, dec_tables *T, bool fu
                                 if (tc > 1 || th > 1 || n > 256 || d + 17 + n > dend) {
                                         return -4;  // baseline: two tables per class
                                 }
-                                if (T && !build_table(*T, tc * 2 + th, d + 1, d + 17, n)) {
+                                if (!kraft_ok(d + 1)) {
                                         return -4;  // over-subscribed Huffman table
                                 }
+                                const int id = tc * 2 + th;  // a new definition: the slot of the old one stays with the scans that used it
+                                memcpy(P.hd.bits[id], d + 1, 16), memcpy(P.hd.vals[id], d + 17, n);
+                                P.hd.n[id] = n, P.hd.defined[id] = true, P.hd.slot[id] = -1;
                                 d += 17 + n;
                         }
                 } else if (mk == 0xC0) {
@@ -897,6 +954,9 @@ int parse_stream(const uint8_t *s, size_t len, parsed &P, dec_tables *T, bool fu
                         for (int i = 0; i < g.ncomp; ++i) {  // four components: every one sampled 1x1 (no subsampled alpha)
                                 dec_comp &c = g.c[i];
                                 if (c.h < 1 || c.h > 2 || c.v < 1 || c.v > 2 || ((i > 0 || g.ncomp == 4) && (c.h != 1 || c.v != 1)) || c.tq > 3) {
+                                        return -4;
+                                }
+                                if (c.v > c.h) {  // luma 1x2 (4:4:0): no output layout packs it (UYVY and the 4:4:4 packers would read chroma rows that do not exist)
                                         return -4;
                                 }
                                 c.bw = (g.w + 8 * g.hmax - 1) / (8 * g.hmax) * c.h, c.bh = (g.h + 8 * g.vmax - 1) / (8 * g.vmax) * c.v;
@@ -936,9 +996,13 @@ int parse_stream(const uint8_t *s, size_t len, parsed &P, dec_tables *T, bool fu
                                                 S.comp[i] = j;
                                         }
                                 }
-                                S.td[i] = d[2 + 2 * i] >> 4, S.ta[i] = d[2 + 2 * i] & 15;
-                                if (S.comp[i] < 0 || S.td[i] > 1 || S.ta[i] > 1 || !P.have_q[g.c[S.comp[i]].tq]) {
+                                const int td = d[2 + 2 * i] >> 4, ta = d[2 + 2 * i] & 15;
+                                if (S.comp[i] < 0 || td > 1 || ta > 1 || !P.have_q[g.c[S.comp[i]].tq]) {
                                         return -4;
+                                }
+                                S.td[i] = table_slot(P.hd, T, td), S.ta[i] = table_slot(P.hd, T, 2 + ta);
+                                if (S.td[i] < 0 || S.ta[i] < 0) {
+                                        return -4;  // an undefined table, or more table definitions in use than a valid stream has
                                 }
                         }
                         int mcuy;
@@ -1239,10 +1303,13 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
                         // one scan per component, in component order, is what the first SOS promises (GPUJPEG's RGB streams): scans 2 and 3 are laid out as the
                         // host parser would lay them out, their table selectors come from the device, and the device checks the promise
                         dec_geom &g = P.g;
+                        for (int id = 0; id < 4; ++id) {  // the kernel reads table id k of scans 2 and 3 from slot k: the first scan took slots by id
+                                table_slot(P.hd, H.tables, id);
+                        }
                         for (int j = 1; j < 3; ++j) {
                                 dec_scan &S = g.s[j];
                                 const dec_comp &c = g.c[j];
-                                S.ns = 1, S.comp[0] = j, S.td[0] = S.ta[0] = 0;
+                                S.ns = 1, S.comp[0] = j, S.td[0] = 0, S.ta[0] = 2;  // table slots: the kernel takes the selectors from the device
                                 S.mcux = ((g.w * c.h + g.hmax - 1) / g.hmax + 7) / 8;
                                 S.nmcu = S.mcux * (((g.h * c.v + g.vmax - 1) / g.vmax + 7) / 8);
                                 S.seg0 = g.s[j - 1].seg0 + g.s[j - 1].nseg;
@@ -1254,6 +1321,7 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
                 if (!device_scan) {  // start over on the host path (tables and geometry are rebuilt there)
                         P.g = dec_geom{}, P.adobe = -1, P.have_sof = false;
                         memset(P.have_q, 0, sizeof P.have_q);
+                        P.hd = huff_defs{};
                         memset(H.tables, 0, sizeof(dec_tables));
                         memcpy(H.tables->zz, kZigzag, 64);
                 }
@@ -1289,6 +1357,10 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
                 return rc;
         }
         lap("parse");
+        P.g.ntables = multi ? 4 : 0;  // multi: scans 2 and 3 take their selectors from the device, any of slots 0..3 (zeroed when undefined)
+        for (int k = 0; k < kTables; ++k) {
+                P.g.ntables = P.hd.taken[k] ? k + 1 : P.g.ntables;
+        }
         const dec_geom &g = P.g;
         const size_t nseg = multi ? (size_t) (g.s[2].seg0 + g.s[2].nseg) : device_scan ? (size_t) g.s[0].nseg : P.seg_begin.size();
         d->last_nseg = nseg;
