@@ -111,5 +111,26 @@ for codec, w, h in ([] if ONLY == "staged" else ((2, 320, 200), (12, 200, 120), 
             except RuntimeError:
                 pass
             n += 1
+# LDGM FEC: encode from host (packets of 4-, 8- and 16-byte words) and from a device frame at offsets 4 and 1 into a tight device buffer;
+# decode with losses peeling can repair (several levels) and with losses it cannot
+import ldgm_cases as lc
+for k, m, c in ([] if ONLY in ("jpeg", "staged") else ((64, 64, 2), (512, 384, 5))):
+    coder = api.LdgmCoder(lc.matrix(k, m, c, 1), k, m)
+    for size in (1, 4 * k * 3 - 12, 4 * k * 4 - 8, 20_011):
+        frame = util.rng_bytes(size, size)
+        enc_h = coder.encode(frame, b"hdr")
+        for off in (4, 1):
+            dev = torch.zeros(size + 8, dtype=torch.uint8, device="cuda")
+            dev[off:off + size] = torch.from_numpy(frame).cuda()
+            tight = torch.empty(enc_h.size, dtype=torch.uint8, device="cuda")
+            coder.encode(dev[off:off + size], b"hdr", out=tight)
+        n += 3
+        ps = lc.layout(k, 3 + size)[1]
+        rng = np.random.default_rng(size)
+        for loss in (0.1, 0.3, 0.7):
+            buf = enc_h.copy()
+            coder.decode(buf, lc.packets_received(k + m, ps, rng.random(k + m) >= loss))
+            n += 1
+    coder.close()
 torch.cuda.synchronize()
 print("exercised", n, "calls")

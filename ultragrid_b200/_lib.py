@@ -108,6 +108,15 @@ SIGNATURES = {
     "ugb200_jpeg_decoder_expect": (_i, [_vp, _i, _i]),
     "ugb200_jpeg_decode": (_i, [_vp, _vp, _sz, _vp, _i, _l, _i, _i, _i, _i]),
     "ugb200_jpeg_debug_coefficients": (_i, [_vp, ctypes.POINTER(_vp), ctypes.POINTER(_sz)]),
+    # include/ugb200_ldgm.h
+    "ugb200_ldgm_create": (_vp, [_vp]),
+    "ugb200_ldgm_destroy": (None, [_vp]),
+    "ugb200_ldgm_set_matrix": (_i, [_vp, _vp, _i, _i, _i]),
+    "ugb200_ldgm_buffer_size": (_l, [_vp, _i, ctypes.POINTER(_i)]),
+    "ugb200_ldgm_encode": (_i, [_vp, _vp, _vp, _i]),
+    "ugb200_ldgm_encode_frame": (_i, [_vp, _vp, _i, _vp, _i, _vp, _sz, ctypes.POINTER(_i)]),
+    "ugb200_ldgm_encode_device": (_i, [_vp, _vp, _i, _vp, _i, _vp, _sz, ctypes.POINTER(_i)]),
+    "ugb200_ldgm_decode": (_i, [_vp, _vp, _i, _vp, _i, ctypes.POINTER(_i)]),
     # include/ugb200_lavc.h
     "ugb200_to_lavc_supported": (_i, [_i, _i]),
     "ugb200_to_lavc_convert": (_i, [_i, _i, _vp, _vp, _i, _i, _vp]),

@@ -379,3 +379,79 @@ class JpegDecoder:
         out = np.zeros(nbytes, dtype=np.uint8)
         _check(_L.ugb200_jpeg_decode(self._h, buf, len(stream), ctypes.c_void_p(out.ctypes.data), 0, ls, int(out_codec), *shifts), "ugb200_jpeg_decode")
         return out
+
+
+class LdgmCoder:
+    """ugb200_ldgm_* (include/ugb200_ldgm.h): LDGM FEC of the reference's LDGM_session (ldgm/src/ldgm-session.h), on the GPU.
+    ``pcm`` is the compact parity-check matrix as set_pcMatrix reads it: an int32 array of m rows of w_f entries."""
+
+    def __init__(self, pcm, k, m, stream=None):
+        self._stream = stream if stream is not None else torch.cuda.current_stream()
+        self._h = _L.ugb200_ldgm_create(ctypes.c_void_p(self._stream.cuda_stream))
+        if not self._h:
+            raise RuntimeError("ugb200_ldgm_create failed")
+        self.set_matrix(pcm, k, m)
+
+    def set_matrix(self, pcm, k, m):
+        import numpy as np
+        pcm = np.ascontiguousarray(pcm, dtype=np.int32).reshape(m, -1)
+        _check(_L.ugb200_ldgm_set_matrix(self._h, ctypes.c_void_p(pcm.ctypes.data), k, m, pcm.shape[1]), "ugb200_ldgm_set_matrix")
+        self.k, self.m = k, m
+
+    def close(self):
+        if self._h and _L is not None:
+            _L.ugb200_ldgm_destroy(self._h)
+        self._h = None
+
+    def __del__(self):
+        self.close()
+
+    def buffer_size(self, payload_size):
+        """(encoded length, packet size) for a header + frame of payload_size bytes"""
+        ps = ctypes.c_int()
+        n = _L.ugb200_ldgm_buffer_size(self._h, payload_size, ctypes.byref(ps))
+        if n < 0:
+            raise RuntimeError(f"ugb200_ldgm_buffer_size failed with code {n}")
+        return n, ps.value
+
+    def encode(self, frame, hdr=b"", out=None):
+        """encode_hdr_frame.  ``frame`` is bytes / a uint8 numpy array (host) or a uint8 CUDA tensor (device, may be a view at any
+        offset); returns a uint8 numpy array, or for a device frame a CUDA tensor (``out`` may supply either).  A device encode is
+        asynchronous and ordered after, and before, the work of the current torch stream."""
+        import numpy as np
+        hdr = bytes(hdr)
+        n_out = ctypes.c_int()
+        if isinstance(frame, torch.Tensor):
+            total, _ = self.buffer_size(len(hdr) + frame.numel())
+            if out is None:
+                out = torch.empty(total, dtype=torch.uint8, device=frame.device)
+            # the coder runs on its own stream: it starts after the work queued so far on the caller's stream (which made the frame),
+            # and the caller's stream continues after the encode; the allocator keeps both tensors until the coder's stream is done
+            caller = torch.cuda.current_stream(frame.device)
+            if caller != self._stream:
+                self._stream.wait_stream(caller)
+            _check(_L.ugb200_ldgm_encode_device(self._h, hdr, len(hdr), _ptr(frame), frame.numel(), _ptr(out), out.numel(),
+                                                ctypes.byref(n_out)), "ugb200_ldgm_encode_device")
+            if caller != self._stream:
+                frame.record_stream(self._stream)
+                out.record_stream(self._stream)
+                caller.wait_stream(self._stream)
+            return out[:n_out.value]
+        src = np.frombuffer(frame, dtype=np.uint8) if isinstance(frame, (bytes, bytearray)) else np.ascontiguousarray(frame, dtype=np.uint8)
+        total, _ = self.buffer_size(len(hdr) + src.size)
+        if out is None:
+            out = np.empty(total, dtype=np.uint8)
+        _check(_L.ugb200_ldgm_encode_frame(self._h, hdr, len(hdr), ctypes.c_void_p(src.ctypes.data), src.size, ctypes.c_void_p(out.ctypes.data),
+                                           out.size, ctypes.byref(n_out)), "ugb200_ldgm_encode_frame")
+        return out[:n_out.value]
+
+    def decode(self, buf, ranges):
+        """decode_frame on a writable uint8 numpy array, in place; ``ranges`` is a dict or a list of (offset, length) of received bytes.
+        Returns the frame size of the header (the payload starts at buf[4:]), or 0 when the frame cannot be recovered."""
+        import numpy as np
+        items = list(ranges.items()) if isinstance(ranges, dict) else list(ranges)
+        r = np.ascontiguousarray(np.array(items, dtype=np.int32).reshape(-1, 2))
+        fs = ctypes.c_int()
+        _check(_L.ugb200_ldgm_decode(self._h, ctypes.c_void_p(buf.ctypes.data), buf.size, ctypes.c_void_p(r.ctypes.data), len(items),
+                                     ctypes.byref(fs)), "ugb200_ldgm_decode")
+        return fs.value
