@@ -128,6 +128,20 @@ UGB_API long ugb200_jpeg_debug_segments(const uint8_t *stream, size_t len, uint3
  * decoder creation forces one way (device: at any size).  The stream is uploaded on a copy stream of the decoder, under the kernels of the frame before.
  * ugb200_jpeg_decoder_last_segments returns the segment table of the last decode as the device holds it (waits for the decoder's stream). */
 UGB_API long ugb200_jpeg_decoder_last_segments(ugb200_jpeg_decoder *dec, uint32_t *begin, uint32_t *end, long cap);
+/* Huffman decoding.  A restart segment of fewer than 64 MCUs is decoded by one GPU thread.  Longer segments - every scan of a stream without DRI (RTSP
+ * cameras, webcam MJPEG, libjpeg's defaults) - take a self-synchronising route: the segment's bytes are cut into subsequences of 64 bytes, one thread
+ * each; every thread decodes from a guessed state until its exit state (bit position, block of the MCU, zig-zag position at the first symbol boundary
+ * behind the next subsequence's start) stops changing from round to round, which proves every start state; a prefix sum of block counts and DC
+ * differences then places the blocks.  Both routes give the same coefficients for any bytes, damaged ones included (DESIGN.md section 2).
+ * ugb200_jpeg_decoder_last_sync reports what the last decode did (waits for the decoder's stream): the scans that took the self-synchronising route
+ * (0: none), its subsequences over all segments and its rounds.  Test hook, read at decoder creation: UGB200_JPEG_SYNC=off forces one thread per
+ * segment, UGB200_JPEG_SYNC=on[:<bytes>] forces the self-synchronising route for every stream, optionally with another subsequence length. */
+struct ugb200_jpeg_sync_stats {
+        int scans;           /* scans of the last decode that took the self-synchronising route */
+        int rounds;          /* synchronisation rounds (1: every guessed start state was right at once) */
+        long subsequences;   /* subsequences over all restart segments of those scans */
+};
+UGB_API int ugb200_jpeg_decoder_last_sync(ugb200_jpeg_decoder *dec, struct ugb200_jpeg_sync_stats *st);
 UGB_API ugb200_jpeg_decoder *ugb200_jpeg_decoder_create(cuda_wrapper_stream_t stream);   /* gpujpeg_decoder_create, gpujpeg.c:93 */
 UGB_API void ugb200_jpeg_decoder_destroy(ugb200_jpeg_decoder *dec);                      /* gpujpeg_decoder_destroy */
 /* The destination of ugb200_jpeg_decode is sized by the CALLER (video_desc of reconfigure(), gpujpeg.c:176-203) while the stream's SOF0

@@ -111,6 +111,29 @@ for codec, w, h in ([] if ONLY == "staged" else ((2, 320, 200), (12, 200, 120), 
             except RuntimeError:
                 pass
             n += 1
+# JPEG decoder, self-synchronising Huffman route: a no-DRI 4:2:0 stream (default subsequences and 8-byte ones), truncated, and the adversarial stream
+# of tests/test_jpeg_decode_sync.py (many rounds)
+if ONLY != "staged":
+    import io
+    from PIL import Image
+    from test_jpeg import natural_rgb
+    from test_jpeg_decode_sync import adversarial_stream
+    b = io.BytesIO()
+    Image.fromarray(natural_rgb(333, 211, 4)).save(b, "JPEG", quality=90, subsampling=2)
+    s420 = b.getvalue()
+    os.environ.pop("UGB200_JPEG_MARKER_SCAN", None)
+    for sync in ("on", "on:8"):
+        os.environ["UGB200_JPEG_SYNC"] = sync
+        dec3 = api.JpegDecoder()
+        for data in (s420, s420[:len(s420) // 2], adversarial_stream()):
+            for out_c in (2, 29):
+                try:
+                    dec3.decode(data, out_c)
+                except RuntimeError:
+                    pass
+                n += 1
+        dec3.close()
+    os.environ.pop("UGB200_JPEG_SYNC", None)
 # LDGM FEC: encode from host (packets of 4-, 8- and 16-byte words) and from a device frame at offsets 4 and 1 into a tight device buffer;
 # decode with losses peeling can repair (several levels) and with losses it cannot
 import ldgm_cases as lc

@@ -103,6 +103,7 @@ SIGNATURES = {
     "ugb200_jpeg_get_image_info": (_i, [_vp, _sz, _vp]),
     "ugb200_jpeg_debug_segments": (_l, [_vp, _sz, _vp, _vp, _l]),
     "ugb200_jpeg_decoder_last_segments": (_l, [_vp, _vp, _vp, _l]),
+    "ugb200_jpeg_decoder_last_sync": (_i, [_vp, _vp]),
     "ugb200_jpeg_decoder_create": (_vp, [_vp]),
     "ugb200_jpeg_decoder_destroy": (None, [_vp]),
     "ugb200_jpeg_decoder_expect": (_i, [_vp, _i, _i]),

@@ -341,6 +341,10 @@ def jpeg_image_info(stream):
     return info
 
 
+class JpegSyncStats(ctypes.Structure):
+    _fields_ = [("scans", ctypes.c_int), ("rounds", ctypes.c_int), ("subsequences", ctypes.c_long)]
+
+
 class JpegDecoder:
     """ugb200_jpeg_decode*: the stage src/video_decompress/gpujpeg.c delegates to libgpujpeg."""
 
@@ -357,6 +361,12 @@ class JpegDecoder:
 
     def __del__(self):
         self.close()
+
+    def last_sync(self):
+        """what the last decode's self-synchronising Huffman route did: {"scans", "subsequences", "rounds"} (scans 0: one thread per restart segment)"""
+        st = JpegSyncStats()
+        _check(_L.ugb200_jpeg_decoder_last_sync(self._h, ctypes.byref(st)), "ugb200_jpeg_decoder_last_sync")
+        return {"scans": st.scans, "subsequences": st.subsequences, "rounds": st.rounds}
 
     def decode(self, stream, out_codec, shifts=(0, 8, 16), device=False, pitch=0, out=None, sync=True):
         """bytes -> numpy array (host) or CUDA tensor (device=True) holding height rows of vc_get_linesize(width, out_codec) bytes"""

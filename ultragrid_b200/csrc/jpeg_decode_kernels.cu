@@ -9,12 +9,15 @@
 //                           table per Huffman table in shared memory (longer codes: min/max-code walk), DC prediction; every block is
 //                           built in shared memory and written as 128 bytes into the int16 [block][64] buffer (or, when the scans do
 //                           not cover every block, scattered into a cleared buffer)
+//   K1'    jpeg_sync_table_kernel, jpeg_sync_kernel, jpeg_sync_write_kernel   instead of K1 for restart segments of at least kSyncMinMcus MCUs
+//                           (every scan without DRI): self-synchronising decoding, one thread per kSyncBytes of entropy-coded data, the same
+//                           coefficients as K1 for any bytes (both use jpeg_huffman_step.cuh; see the comment above jpeg_sync_kernel)
 //   K2     jpeg_idct_kernel one thread per 8x8 block: dequantise, float AAN inverse DCT (fixed operation order = bit-exact with
 //                           oracle/jpeg_decode_oracle.c), level shift, clamp, 8 x 8-byte stores into the component plane
 //   pack   the component planes go through the from_planar kernels that already exist (planar_conv_kernels.cu):
 //                           4:2:2 -> UYVY (yuv422p_to_uyvy), 4:2:0 -> UYVY (yuv420p_to_uyvy), 4:4:4 YCbCr -> VUYA (yuv444p_to_vuya),
 //                           RGB -> RGB (rgbpXX_to_rgb), then ugb200_pixfmt_convert when another output codec was asked for.
-// Restart intervals are the unit of parallelism; a stream without DRI decodes correctly but on one thread per scan.
+// Restart intervals are the unit of parallelism of K1; K1' does not depend on them.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -35,47 +38,18 @@
 #include "../../include/ugb200.h"
 #include "../../include/ugb200_jpeg.h"
 #include "jpeg_marker_bounds.cuh"
+#include "jpeg_huffman_step.cuh"
 #include "../../include/cuda_wrapper.h"
+
+#include <cooperative_groups.h>
+
+namespace cg = cooperative_groups;
 
 namespace ugb {
 
 static const uint8_t kZigzag[64] = { 0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
                                      41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
                                      30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63 };
-
-constexpr int kLook = 9;
-/// Huffman table slots.  A DHT definition is built into a slot when a scan first uses it: table id k (DC Th 0, 1 = 0, 1; AC Th 0, 1 = 2, 3)
-/// goes to slot k when that slot is free, otherwise to the lowest free one.  A table redefined between scans (T.81 B.2.4.2) thus gets a slot
-/// of its own, and every scan keeps the tables it was coded with.  In a valid stream each component appears in one scan and uses one DC and
-/// one AC table, and only definitions that a scan uses take a slot: four components never need more than eight.
-constexpr int kTables = 8;
-
-struct dec_tables {
-        uint16_t lut[kTables][1 << kLook];  // (length << 8) | symbol for codes of up to kLook bits, 0 = longer code
-        int maxcode[kTables][18];           // T.81 F.2.2.3, -1 = no code of that length
-        int valoff[kTables][17];            // valptr - mincode
-        uint8_t vals[kTables][256];
-        uint8_t zz[64];
-        float m[4][64];               // dequantisation x AAN scale, natural order
-};
-
-struct dec_comp {
-        int h, v, tq;
-        int bw, bh;     // blocks per row / rows of the padded plane
-        int blk_off;    // first block of the component in the coefficient buffer
-        long plane_off; // first byte of the plane in the plane buffer
-};
-struct dec_scan {
-        int ns, comp[4], td[4], ta[4];  // td, ta: table slots of dec_tables
-        int mcux, nmcu;
-        int seg0, nseg;  // segments [seg0, seg0 + nseg)
-};
-struct dec_geom {
-        int w, h, ncomp, hmax, vmax, ri, nscans, nblocks;  // ncomp 3, or 4 (R G B A, all 1x1)
-        int ntables;  // Huffman table slots in use: [0, ntables) (the Huffman kernel copies only those to shared memory)
-        dec_comp c[4];
-        dec_scan s[4];
-};
 
 struct bit_reader {  // MSB-first, removes stuffed zero bytes, feeds zeros beyond `end`
         const uint8_t *p, *end;
@@ -124,31 +98,6 @@ struct bit_reader {  // MSB-first, removes stuffed zero bytes, feeds zeros beyon
         __device__ __forceinline__ void skip(int n) { acc <<= n, nbits -= n; }
 };
 
-__device__ __forceinline__ int decode_symbol(bit_reader &r, const dec_tables *t, int tab)
-{
-        const uint32_t e = t->lut[tab][r.peek(kLook)];
-        if (e) {
-                r.skip(e >> 8);
-                return e & 0xff;
-        }
-        const uint32_t v16 = r.peek(16);
-        for (int l = kLook + 1; l <= 16; ++l) {
-                const int code = (int) (v16 >> (16 - l));
-                if (code <= t->maxcode[tab][l]) {
-                        r.skip(l);
-                        return t->vals[tab][t->valoff[tab][l] + code];
-                }
-        }
-        r.skip(16);
-        return 0;  // corrupt stream
-}
-__device__ __forceinline__ int receive_extend(bit_reader &r, int n)  // F.2.2.1, n in 1..15
-{
-        const int v = (int) r.peek(n);
-        r.skip(n);
-        return v < (1 << (n - 1)) ? v - (1 << n) + 1 : v;
-}
-
 /// FULL: every block of the coefficient array is decoded by exactly one thread (the host checks: every component in a scan, the scans' MCU grids equal to the
 /// padded planes) - the thread then builds its block in shared memory ([word][thread]: conflict-free, dynamically indexable) and writes all 128 bytes of it,
 /// so the array needs no clearing beforehand (133 MB at 8K) and the scattered 2-byte stores become whole-line stores.  !FULL: sparse stores into a cleared array.
@@ -162,6 +111,80 @@ __device__ __forceinline__ void copy_words(void *dst, const void *src, int bytes
                 ((uint32_t *) dst)[i] = ((const uint32_t *) src)[i];
         }
 }
+/// what the Huffman kernels read of the tables: the slots in use and the zig-zag order (not the dequantisation multipliers)
+__device__ __forceinline__ void copy_tables(dec_tables *t, const dec_tables *tables, int ntables)
+{
+        copy_words(t->lut, tables->lut, ntables * (int) sizeof t->lut[0]);
+        copy_words(t->maxcode, tables->maxcode, ntables * (int) sizeof t->maxcode[0]);
+        copy_words(t->valoff, tables->valoff, ntables * (int) sizeof t->valoff[0]);
+        copy_words(t->vals, tables->vals, ntables * (int) sizeof t->vals[0]);
+        copy_words(t->zz, tables->zz, (int) sizeof t->zz);
+}
+constexpr size_t kTablesSmem = (sizeof(dec_tables) + 15) & ~(size_t) 15;
+
+/// where decode_block puts a block: FULL - the thread's column of shared memory, written out as 128 bytes by finish(); !FULL - the non-zero coefficients
+/// straight into the cleared array.  Padding blocks of an MCU (`inside` false) are decoded and not stored.
+template <bool FULL>
+struct block_sink {
+        uint32_t *col;
+        int16_t *blk;
+        const uint8_t *zz;
+        bool inside;
+        __device__ __forceinline__ void begin()
+        {
+                if (FULL) {
+#pragma unroll
+                        for (int w = 0; w < 32; ++w) {
+                                col[w * kHuffThreads] = 0;
+                        }
+                }
+        }
+        __device__ __forceinline__ void dc(uint32_t pred)
+        {
+                if (FULL) {
+                        col[0] = pred & 0xffffu;
+                } else if (inside && pred != 0) {
+                        blk[0] = (int16_t) pred;
+                }
+        }
+        __device__ __forceinline__ void operator()(int i, int v)
+        {
+                const int n = zz[i];
+                if (FULL) {
+                        ((int16_t *) (col + (n >> 1) * kHuffThreads))[n & 1] = (int16_t) v;
+                } else if (inside) {
+                        blk[n] = (int16_t) v;
+                }
+        }
+        __device__ __forceinline__ void finish()
+        {
+                if (FULL && inside) {
+#pragma unroll
+                        for (int q = 0; q < 8; ++q) {
+                                ((uint4 *) blk)[q] = make_uint4(col[(4 * q) * kHuffThreads], col[(4 * q + 1) * kHuffThreads], col[(4 * q + 2) * kHuffThreads], col[(4 * q + 3) * kHuffThreads]);
+                        }
+                }
+        }
+};
+
+/// the scan of restart segment `s` (with the table selectors the device read for the later scans of a multi-scan stream) and its MCUs [m0, m1)
+__device__ __forceinline__ bool segment_scan(const dec_geom &g, int s, const uint32_t *__restrict__ dev_scans, dec_scan &S, int &m0, int &m1)
+{
+        int sc = 0;
+        while (sc < g.nscans && s >= g.s[sc].seg0 + g.s[sc].nseg) {
+                ++sc;
+        }
+        if (sc >= g.nscans) {
+                return false;
+        }
+        S = g.s[sc];
+        if (dev_scans != nullptr && sc > 0) {  // multi-scan stream with the marker scan on the device: the SOS headers of the later scans were read there
+                S.td[0] = (int) dev_scans[kMetaBounds + 6 * sc + 4], S.ta[0] = 2 + (int) dev_scans[kMetaBounds + 6 * sc + 5];  // no DHT between the scans
+        }
+        const int ls = s - S.seg0;
+        m0 = g.ri ? ls * g.ri : 0, m1 = g.ri ? min(m0 + g.ri, S.nmcu) : S.nmcu;
+        return true;
+}
 
 template <bool FULL>
 __global__ void __launch_bounds__(kHuffThreads) jpeg_decode_huffman_kernel(const uint8_t *__restrict__ stream, const uint32_t *__restrict__ seg_begin,
@@ -170,31 +193,18 @@ __global__ void __launch_bounds__(kHuffThreads) jpeg_decode_huffman_kernel(const
 {
         extern __shared__ uint8_t smem_raw[];
         dec_tables *t = (dec_tables *) smem_raw;
-        uint32_t *const col = (uint32_t *) (smem_raw + ((sizeof(dec_tables) + 15) & ~(size_t) 15)) + threadIdx.x;  // FULL: word w of my block at col[w * kHuffThreads]
-        // what this kernel reads: the slots in use and the zig-zag order (not the dequantisation multipliers)
-        copy_words(t->lut, tables->lut, g.ntables * (int) sizeof t->lut[0]);
-        copy_words(t->maxcode, tables->maxcode, g.ntables * (int) sizeof t->maxcode[0]);
-        copy_words(t->valoff, tables->valoff, g.ntables * (int) sizeof t->valoff[0]);
-        copy_words(t->vals, tables->vals, g.ntables * (int) sizeof t->vals[0]);
-        copy_words(t->zz, tables->zz, (int) sizeof t->zz);
+        uint32_t *const col = (uint32_t *) (smem_raw + kTablesSmem) + threadIdx.x;  // FULL: word w of my block at col[w * kHuffThreads]
+        copy_tables(t, tables, g.ntables);
         __syncthreads();
         const int s = blockIdx.x * blockDim.x + threadIdx.x;
-        int sc = 0;
-        while (sc < g.nscans && s >= g.s[sc].seg0 + g.s[sc].nseg) {
-                ++sc;
-        }
-        if (sc >= g.nscans) {
+        dec_scan S;
+        int m0, m1;
+        if (!segment_scan(g, s, dev_scans, S, m0, m1)) {
                 return;
         }
-        dec_scan S = g.s[sc];
-        if (dev_scans != nullptr && sc > 0) {  // multi-scan stream with the marker scan on the device: the SOS headers of the later scans were read there
-                S.td[0] = (int) dev_scans[kMetaBounds + 6 * sc + 4], S.ta[0] = 2 + (int) dev_scans[kMetaBounds + 6 * sc + 5];  // no DHT between the scans
-        }
-        const int ls = s - S.seg0;
-        const int m0 = g.ri ? ls * g.ri : 0, m1 = g.ri ? min(m0 + g.ri, S.nmcu) : S.nmcu;
         bit_reader r = { stream + seg_begin[s], stream + seg_end[s], 0, 0, nullptr, 0, 0 };
         r.prime();
-        int pred[4] = { 0, 0, 0, 0 };
+        uint32_t pred[4] = { 0, 0, 0, 0 };
         for (int m = m0; m < m1; ++m) {
                 const int mx = m % S.mcux, my = m / S.mcux;
                 for (int k = 0; k < S.ns; ++k) {
@@ -203,56 +213,299 @@ __global__ void __launch_bounds__(kHuffThreads) jpeg_decode_huffman_kernel(const
                         for (int by = 0; by < nv; ++by) {
                                 for (int bx = 0; bx < nh; ++bx) {
                                         const int X = mx * nh + bx, Y = my * nv + by;
-                                        const bool inside = X < c.bw && Y < c.bh;
-                                        int16_t *blk = coef + ((long) c.blk_off + (long) Y * c.bw + X) * 64;
-                                        if (FULL) {
-#pragma unroll
-                                                for (int w = 0; w < 32; ++w) {
-                                                        col[w * kHuffThreads] = 0;
-                                                }
-                                        }
-                                        r.refill();
-                                        const int tt = decode_symbol(r, t, S.td[k]);
-                                        r.refill();
-                                        if (tt) {
-                                                pred[k] += receive_extend(r, tt & 15);
-                                        }
-                                        if (FULL) {
-                                                col[0] = (uint32_t) pred[k] & 0xffffu;
-                                        } else if (inside && pred[k] != 0) {
-                                                blk[0] = (int16_t) pred[k];
-                                        }
-                                        for (int i = 1; i < 64;) {
-                                                r.refill();
-                                                const int rs = decode_symbol(r, t, S.ta[k]), run = rs >> 4, sz = rs & 15;
-                                                if (sz == 0) {
-                                                        if (run != 15) {
-                                                                break;  // EOB
-                                                        }
-                                                        i += 16;
-                                                        continue;
-                                                }
-                                                i += run;
-                                                const int v = receive_extend(r, sz);  // refill guarantees >= 33 bits: 16 + 15 fit
-                                                if (FULL) {
-                                                        if (i < 64) {
-                                                                const int n = t->zz[i];
-                                                                ((int16_t *) (col + (n >> 1) * kHuffThreads))[n & 1] = (int16_t) v;
-                                                        }
-                                                } else if (i < 64 && inside) {
-                                                        blk[t->zz[i]] = (int16_t) v;
-                                                }
-                                                ++i;
-                                        }
-                                        if (FULL && inside) {
-#pragma unroll
-                                                for (int q = 0; q < 8; ++q) {
-                                                        ((uint4 *) blk)[q] = make_uint4(col[(4 * q) * kHuffThreads], col[(4 * q + 1) * kHuffThreads], col[(4 * q + 2) * kHuffThreads], col[(4 * q + 3) * kHuffThreads]);
-                                                }
-                                        }
+                                        block_sink<FULL> sink = { col, coef + ((long) c.blk_off + (long) Y * c.bw + X) * 64, t->zz, X < c.bw && Y < c.bh };
+                                        sink.begin();
+                                        decode_block(r, t, S.td[k], S.ta[k], pred[k], sink);
+                                        sink.finish();
                                 }
                         }
                 }
+        }
+}
+
+// ---- the self-synchronising route (segments of many MCUs; every scan without DRI) -------------------------------------------------------------------
+// A segment's bytes are cut into subsequences of `sub` bytes, one thread each (Weißenberger & Schmidt, ICPP 2018).  A subsequence's entry is the decoder
+// state (bit address, block of the MCU, zig-zag position) at the first symbol boundary at or after its start.  The first subsequence of a segment knows its
+// entry; the others start from a guess.
+//   jpeg_sync_table_kernel  subsequences per segment (from the segment table, so the device marker scan needs no host round trip) and their prefix sum
+//   jpeg_sync_kernel        cooperative grid.  Round r: every subsequence whose entry changed decodes from it to its exit - the first symbol boundary at or
+//                           after the next subsequence's start - counting the blocks whose DC symbol starts inside and their DC differences per component
+//                           (walk_count); an exit that differs from the next entry replaces it.  A round without a change ends the loop: then every
+//                           entry is the exit of its predecessor, proved from the segment's start (after round r the first r + 1 are proved, so at most
+//                           one round per subsequence).  Then an exclusive scan of the counts and sums over all subsequences (uint32, wrapping).
+//   jpeg_sync_write_kernel  one thread per subsequence: from its proved entry, the rest of a block begun before (not stored), then every block whose DC
+//                           symbol starts inside, each decoded whole (read past the end as far as it needs) with decode_block and stored as the
+//                           restart-segment kernel stores it; block index and DC predictors = the scan minus the value at the segment's first subsequence.
+//                           Blocks past the segment's MCUs are dropped; the last subsequence goes on into the zero tail until they are all there.
+constexpr int kSyncThreads = 128;
+/// subsequence length in bytes (the default; UGB200_JPEG_SYNC=on:<bytes> sets another at decoder creation): 64 B give an 8K q90 frame ~80 000
+/// threads, about 60 % of what the cooperative grid holds at once; it is the only length timed so far (DESIGN.md section 4.1)
+constexpr int kSyncBytes = 64;
+constexpr int kSyncVals = 5;
+/// restart intervals of at least this many MCUs take the self-synchronising route (chosen from tools/jpeg_nodri_bench.py, DESIGN.md section 4)
+constexpr int kSyncMinMcus = 64;  // per subsequence: blocks, DC sums of the scan components 0..3
+
+struct sync_bufs {
+        uint32_t *sub_first;  // [nseg + 1]: first subsequence of each segment, total at [nseg]
+        sync_point *entry, *exitp;
+        uint32_t *res, *scan;  // [kSyncVals][nsub]
+        uint32_t *dirty;       // entry changed in the last round
+        uint32_t *cta;         // [kSyncVals][grid] CTA totals
+        uint32_t *ctr;         // [3] changes per round (rotating), [3] rounds, [4] subsequences
+};
+
+__global__ void __launch_bounds__(1024) jpeg_sync_table_kernel(const uint32_t *__restrict__ seg_begin, const uint32_t *__restrict__ seg_end, int nseg, int sub,
+                                                                 uint32_t *__restrict__ sub_first)
+{
+        __shared__ uint32_t s_w[32];
+        __shared__ uint32_t s_carry;
+        if (threadIdx.x == 0) {
+                s_carry = 0;
+        }
+        __syncthreads();
+        for (int base = 0; base < nseg; base += 1024) {
+                const int i = base + (int) threadIdx.x;
+                const uint32_t v = i < nseg ? (uint32_t) sub_count(seg_end[i] - seg_begin[i], sub) : 0;
+                uint32_t incl = v;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) {
+                        const uint32_t o = __shfl_up_sync(0xffffffffu, incl, d);
+                        if ((threadIdx.x & 31) >= (unsigned) d) {
+                                incl += o;
+                        }
+                }
+                if ((threadIdx.x & 31) == 31) {
+                        s_w[threadIdx.x >> 5] = incl;
+                }
+                __syncthreads();
+                uint32_t before = s_carry;
+                for (int w = 0; w < (int) (threadIdx.x >> 5); ++w) {
+                        before += s_w[w];
+                }
+                if (i < nseg) {
+                        sub_first[i] = before + incl - v;
+                }
+                __syncthreads();
+                if (threadIdx.x == 1023) {
+                        s_carry = before + incl;
+                }
+                __syncthreads();
+        }
+        if (threadIdx.x == 0) {
+                sub_first[nseg] = s_carry;
+        }
+}
+
+/// the segment of subsequence j: the last one whose first subsequence is <= j
+__device__ __forceinline__ int sub_segment(const uint32_t *__restrict__ sub_first, int nseg, uint32_t j)
+{
+        int lo = 0, hi = nseg - 1;
+        while (lo < hi) {
+                const int mid = (lo + hi + 1) >> 1;
+                if (sub_first[mid] <= j) {
+                        lo = mid;
+                } else {
+                        hi = mid - 1;
+                }
+        }
+        return lo;
+}
+
+__device__ __forceinline__ bool same_point(sync_point a, sync_point b) { return a.byte == b.byte && a.tag == b.tag; }
+
+__global__ void __launch_bounds__(kSyncThreads, 8) jpeg_sync_kernel(const uint8_t *__restrict__ stream, const uint32_t *__restrict__ seg_begin,
+                                                                 const uint32_t *__restrict__ seg_end, int nseg, int sub, const dec_tables *__restrict__ tables,
+                                                                 dec_geom g, const uint32_t *__restrict__ dev_scans, sync_bufs B, uint32_t cap)
+{
+        extern __shared__ uint8_t smem_raw[];
+        dec_tables *t = (dec_tables *) smem_raw;
+        __shared__ uint32_t s_w[kSyncThreads / 32][kSyncVals];
+        __shared__ uint32_t s_pre[kSyncVals];
+        copy_tables(t, tables, g.ntables);
+        if (threadIdx.x < kSyncVals) {
+                s_pre[threadIdx.x] = 0;
+        }
+        __syncthreads();
+        cg::grid_group grid = cg::this_grid();
+        const uint32_t nsub = min(B.sub_first[nseg], cap);
+        const uint32_t nthreads = gridDim.x * blockDim.x, gt = blockIdx.x * blockDim.x + threadIdx.x;
+        const uint32_t per = (nsub + nthreads - 1) / nthreads, j0 = min(nsub, gt * per), j1 = min(nsub, j0 + per);
+        // contiguous subsequences per thread: the same ones in every round and in the scan
+        for (uint32_t j = j0; j < j1; ++j) {
+                const int s = sub_segment(B.sub_first, nseg, j);
+                const uint32_t f = B.sub_first[s];
+                B.entry[j] = make_point(sub_start(stream, seg_begin[s], seg_end[s], (int) (j - f), sub), 0, 0);
+                B.dirty[j] = 1;
+                for (int v = 0; v < kSyncVals; ++v) {
+                        B.res[v * cap + j] = 0;
+                }
+        }
+        int round = 0;
+        for (;; ++round) {
+                if (gt == 0) {
+                        B.ctr[(round + 1) % 3] = 0;
+                }
+                for (uint32_t j = j0; j < j1; ++j) {
+                        const int s = sub_segment(B.sub_first, nseg, j);
+                        if (!B.dirty[j] || j + 1 == B.sub_first[s + 1]) {
+                                continue;  // the entry is unchanged, or the last subsequence of its segment (it proves nothing)
+                        }
+                        dec_scan S;
+                        int m0, m1;
+                        segment_scan(g, s, dev_scans, S, m0, m1);
+                        const mcu_layout L = layout_of(g, S);
+                        const sync_point e = B.entry[j];
+                        pos_reader r;
+                        r.s = stream, r.end = seg_end[s];
+                        r.start(e.byte, (int) (e.tag >> 16));
+                        int blk = (e.tag >> 8) & 0xff, zz = e.tag & 0xff;
+                        uint32_t count = 0, sum[4] = { 0, 0, 0, 0 };
+                        const uint64_t limit = sub_start(stream, seg_begin[s], seg_end[s], (int) (j + 1 - B.sub_first[s]), sub);
+                        walk_count(r, t, S.td, S.ta, L, limit, blk, zz, count, sum);
+                        B.exitp[j] = make_point(r.pos(), blk, zz);
+                        B.res[j] = count;
+                        for (int v = 0; v < 4; ++v) {
+                                B.res[(v + 1) * cap + j] = sum[v];
+                        }
+                }
+                grid.sync();
+                uint32_t changed = 0;
+                for (uint32_t j = j0; j < j1; ++j) {
+                        const int s = sub_segment(B.sub_first, nseg, j);
+                        if (j == B.sub_first[s]) {
+                                B.dirty[j] = 0;  // its entry is the segment's start
+                        }
+                        if (j + 1 == B.sub_first[s + 1]) {
+                                continue;
+                        }
+                        // an exit not recomputed this round equals the next entry already: the owner of j + 1 reads dirty[j + 1] only after the grid sync
+                        const bool moved = !same_point(B.exitp[j], B.entry[j + 1]);
+                        if (moved) {
+                                B.entry[j + 1] = B.exitp[j];
+                        }
+                        B.dirty[j + 1] = moved;
+                        changed += moved;
+                }
+                if (changed) {
+                        atomicAdd(B.ctr + round % 3, changed);
+                }
+                grid.sync();
+                if (B.ctr[round % 3] == 0) {
+                        break;
+                }
+        }
+        // exclusive scan of res over all subsequences: thread totals -> CTA -> grid
+        uint32_t tot[kSyncVals] = { 0, 0, 0, 0, 0 };
+        for (uint32_t j = j0; j < j1; ++j) {
+                for (int v = 0; v < kSyncVals; ++v) {
+                        tot[v] += B.res[v * cap + j];
+                }
+        }
+        uint32_t incl[kSyncVals];
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+        for (int v = 0; v < kSyncVals; ++v) {
+                incl[v] = tot[v];
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) {
+                        const uint32_t o = __shfl_up_sync(0xffffffffu, incl[v], d);
+                        if (lane >= d) {
+                                incl[v] += o;
+                        }
+                }
+                if (lane == 31) {
+                        s_w[warp][v] = incl[v];
+                }
+        }
+        __syncthreads();
+        if (threadIdx.x < kSyncVals) {
+                uint32_t c = 0;
+                for (int w = 0; w < kSyncThreads / 32; ++w) {
+                        c += s_w[w][threadIdx.x];
+                }
+                B.cta[threadIdx.x * gridDim.x + blockIdx.x] = c;
+        }
+        grid.sync();
+        for (int v = 0; v < kSyncVals; ++v) {
+                uint32_t c = 0;
+                for (uint32_t b = threadIdx.x; b < blockIdx.x; b += blockDim.x) {
+                        c += B.cta[v * gridDim.x + b];
+                }
+                if (c) {
+                        atomicAdd(s_pre + v, c);
+                }
+        }
+        __syncthreads();
+        uint32_t run[kSyncVals];
+#pragma unroll
+        for (int v = 0; v < kSyncVals; ++v) {
+                run[v] = s_pre[v] + incl[v] - tot[v];
+                for (int w = 0; w < warp; ++w) {
+                        run[v] += s_w[w][v];
+                }
+        }
+        for (uint32_t j = j0; j < j1; ++j) {
+                for (int v = 0; v < kSyncVals; ++v) {
+                        B.scan[v * cap + j] = run[v];
+                        run[v] += B.res[v * cap + j];
+                }
+        }
+        if (gt == 0) {
+                B.ctr[3] = (uint32_t) round + 1, B.ctr[4] = nsub;
+        }
+}
+
+template <bool FULL>
+__global__ void __launch_bounds__(kHuffThreads, 16) jpeg_sync_write_kernel(const uint8_t *__restrict__ stream, const uint32_t *__restrict__ seg_begin,
+                                                                     const uint32_t *__restrict__ seg_end, int nseg, int sub, const dec_tables *__restrict__ tables,
+                                                                     dec_geom g, int16_t *__restrict__ coef, const uint32_t *__restrict__ dev_scans, sync_bufs B,
+                                                                     uint32_t cap)
+{
+        extern __shared__ uint8_t smem_raw[];
+        dec_tables *t = (dec_tables *) smem_raw;
+        uint32_t *const col = (uint32_t *) (smem_raw + kTablesSmem) + threadIdx.x;
+        copy_tables(t, tables, g.ntables);
+        __syncthreads();
+        const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+        if (j >= min(B.sub_first[nseg], cap)) {
+                return;
+        }
+        const int s = sub_segment(B.sub_first, nseg, j);
+        dec_scan S;
+        int m0, m1;
+        if (!segment_scan(g, s, dev_scans, S, m0, m1)) {
+                return;
+        }
+        const mcu_layout L = layout_of(g, S);
+        const uint32_t f = B.sub_first[s], nblk = (uint32_t) (m1 - m0) * (uint32_t) L.bpm;
+        uint32_t idx = B.scan[j] - B.scan[f], pred[4];
+        for (int v = 0; v < 4; ++v) {
+                pred[v] = B.scan[(v + 1) * cap + j] - B.scan[(v + 1) * cap + f];
+        }
+        if (idx >= nblk) {
+                return;
+        }
+        const sync_point e = B.entry[j];
+        pos_reader r;
+        r.s = stream, r.end = seg_end[s];
+        r.start(e.byte, (int) (e.tag >> 16));
+        const int zz = e.tag & 0xff;
+        if (zz) {
+                finish_block(r, t, S.ta[L.k[(e.tag >> 8) & 0xff]], zz);
+        }
+        const bool last = j + 1 == B.sub_first[s + 1];
+        const uint64_t limit = last ? ~(uint64_t) 0 : sub_start(stream, seg_begin[s], seg_end[s], (int) (j + 1 - f), sub);
+        while (idx < nblk && r.pos() < limit) {
+                const int m = m0 + (int) (idx / (uint32_t) L.bpm), b = (int) (idx % (uint32_t) L.bpm), k = L.k[b];
+                const int mx = m % S.mcux, my = m / S.mcux;
+                const dec_comp &c = g.c[S.comp[k]];
+                const int nh = S.ns == 1 ? 1 : c.h, nv = S.ns == 1 ? 1 : c.v;
+                const int X = mx * nh + L.bx[b], Y = my * nv + L.by[b];
+                block_sink<FULL> sink = { col, coef + ((long) c.blk_off + (long) Y * c.bw + X) * 64, t->zz, X < c.bw && Y < c.bh };
+                sink.begin();
+                decode_block(r, t, S.td[k], S.ta[k], pred[k], sink);
+                sink.finish();
+                ++idx;
         }
 }
 
@@ -665,6 +918,13 @@ struct ugb200_jpeg_decoder {
         bool host_once = false; // the device found a multi-scan stream irregular: this frame is repeated with the host parser
         uint32_t *h_flag = nullptr;  // pinned: the device's verdict on a multi-scan stream
         size_t last_nseg = 0;   // segments of the last decode (ugb200_jpeg_decoder_last_segments)
+        // the self-synchronising route: 0 = for segments of at least kSyncMinMcus MCUs (every scan without DRI), 1 = never, 2 = always (UGB200_JPEG_SYNC)
+        int sync_mode = 0, sync_bytes = kSyncBytes;
+        uint32_t *d_sync = nullptr;
+        size_t sync_cap = 0;
+        int sync_grid = 0;       // co-resident CTAs of jpeg_sync_kernel
+        uint32_t *last_sync_ctr = nullptr;  // rounds and subsequences of the last decode on the device (nullptr: the route did not run)
+        int last_sync_scans = 0;
         // pinned staging (the caller's stream buffer is pageable and freed right after the call), two slots: the host side of frame
         // i + 1 (scan, parse, staging copy) runs while the device still works on frame i
         struct host_slot {
@@ -753,27 +1013,6 @@ bool kraft_ok(const uint8_t *bits)
                 code <<= 1;
         }
         return true;
-}
-
-/// the bits / values have passed kraft_ok
-void build_table(dec_tables &t, int tab, const uint8_t *bits, const uint8_t *vals, int n)
-{
-        memset(t.lut[tab], 0, sizeof t.lut[tab]);
-        memcpy(t.vals[tab], vals, n);
-        int code = 0, k = 0;
-        for (int l = 1; l <= 16; ++l) {
-                t.valoff[tab][l] = k - code;
-                for (int i = 0; i < bits[l - 1]; ++i, ++k, ++code) {
-                        if (l <= kLook) {
-                                for (int fill = 0; fill < (1 << (kLook - l)); ++fill) {
-                                        t.lut[tab][(code << (kLook - l)) | fill] = (uint16_t) (l << 8 | vals[k]);
-                                }
-                        }
-                }
-                t.maxcode[tab][l] = bits[l - 1] ? code - 1 : -1;
-                code <<= 1;
-        }
-        t.maxcode[tab][17] = 0x7fffffff;
 }
 
 /// the table slot of the current definition of table id `id`, built on first use (see kTables); -1: the table is undefined or no slot is left
@@ -1168,6 +1407,15 @@ UGB_API ugb200_jpeg_decoder *ugb200_jpeg_decoder_create(cuda_wrapper_stream_t st
         }
         const char *m = getenv("UGB200_JPEG_MARKER_SCAN");  // "host" / "device": force one of the two marker scans (tests, A/B timing)
         d->scan_mode = !m ? 0 : m[0] == 'h' ? 1 : m[0] == 'd' ? 2 : 0;
+        const char *y = getenv("UGB200_JPEG_SYNC");  // test hook: "off" / "on[:<subsequence bytes>]" forces the Huffman route (include/ugb200_jpeg.h)
+        if (y && strncmp(y, "off", 3) == 0) {
+                d->sync_mode = 1;
+        } else if (y && strncmp(y, "on", 2) == 0) {
+                d->sync_mode = 2;
+                if (y[2] == ':' && atoi(y + 3) >= 1) {
+                        d->sync_bytes = atoi(y + 3);
+                }
+        }
         return d;
 }
 
@@ -1182,7 +1430,7 @@ UGB_API void ugb200_jpeg_decoder_destroy(ugb200_jpeg_decoder *d)
                 cudaStreamDestroy(d->copy);
         }
         cudaFree(d->planes), cudaFree(d->native), cudaFree(d->staging), cudaFree(d->coef), cudaFree(d->d_seg), cudaFree(d->d_tables);
-        cudaFree(d->d_marks), cudaFree(d->d_mark_cnt);
+        cudaFree(d->d_marks), cudaFree(d->d_mark_cnt), cudaFree(d->d_sync);
         cudaFreeHost(d->h_flag);
         for (auto &h : d->hs) {
                 if (h.stream) {
@@ -1218,6 +1466,22 @@ UGB_API long ugb200_jpeg_decoder_last_segments(ugb200_jpeg_decoder *d, uint32_t 
                 return -2;
         }
         return n;
+}
+
+UGB_API int ugb200_jpeg_decoder_last_sync(ugb200_jpeg_decoder *d, struct ugb200_jpeg_sync_stats *st)
+{
+        if (!d || !st) {
+                return -1;
+        }
+        if (cudaStreamSynchronize(d->stream) != cudaSuccess) {
+                return -2;
+        }
+        uint32_t c[2] = { 0, 0 };
+        if (d->last_sync_ctr && cudaMemcpy(c, d->last_sync_ctr + 3, 8, cudaMemcpyDeviceToHost) != cudaSuccess) {
+                return -2;
+        }
+        st->scans = d->last_sync_scans, st->rounds = (int) c[0], st->subsequences = (long) c[1];
+        return 0;
 }
 
 UGB_API int ugb200_jpeg_decoder_expect(ugb200_jpeg_decoder *d, int width, int height)
@@ -1451,8 +1715,62 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
                 full = full && seen[0] == 1 && seen[1] == 1 && seen[2] == 1 && (g.ncomp == 3 || seen[3] == 1);
         }
         const unsigned hgrid = (unsigned) ((nseg + kHuffThreads - 1) / kHuffThreads);
-        const size_t hsmem = ((sizeof(dec_tables) + 15) & ~(size_t) 15) + (size_t) kHuffThreads * 128;
-        if (full) {
+        const size_t hsmem = kTablesSmem + (size_t) kHuffThreads * 128;
+        // Huffman route: restart segments of few MCUs keep one thread each; longer ones (every scan without DRI) are decoded by the self-synchronising
+        // route, whose parallelism does not depend on the stream's restart interval.  The segment length in MCUs is the same for every scan of a stream.
+        const bool sync = d->sync_mode == 2 || (d->sync_mode == 0 && (g.ri == 0 || g.ri >= kSyncMinMcus));
+        d->last_sync_ctr = nullptr, d->last_sync_scans = 0;
+        if (sync) {
+                const int sub = d->sync_bytes;
+                const size_t cap = len / (size_t) sub + nseg + 1;  // a segment of n bytes has at most n / sub + 1 subsequences
+                if (d->sync_grid == 0) {
+                        int dev = 0, sms = 0, per_sm = 0;
+                        cudaGetDevice(&dev);
+                        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+                        cudaFuncSetAttribute(jpeg_sync_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) kTablesSmem);
+                        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, jpeg_sync_kernel, kSyncThreads, kTablesSmem);
+                        d->sync_grid = sms * std::max(1, per_sm);
+                }
+                const int grid = (int) std::min((size_t) d->sync_grid, (cap + kSyncThreads - 1) / kSyncThreads);
+                const size_t words = (nseg + 1) + 4 * cap + 2 * kSyncVals * cap + cap + (size_t) kSyncVals * grid + 8;
+                if (cap > 0xFFFFFFF0u || !dgrow(d->d_sync, d->sync_cap, words)) {
+                        return -2;
+                }
+                sync_bufs B;
+                uint32_t *w = d->d_sync;
+                B.sub_first = w, w += nseg + 1;
+                B.entry = (sync_point *) w, w += 2 * cap;
+                B.exitp = (sync_point *) w, w += 2 * cap;
+                B.res = w, w += kSyncVals * cap;
+                B.scan = w, w += kSyncVals * cap;
+                B.dirty = w, w += cap;
+                B.cta = w, w += (size_t) kSyncVals * grid;
+                B.ctr = w;
+                cudaMemsetAsync(B.ctr, 0, 8 * 4, s);
+                jpeg_sync_table_kernel<<<1, 1024, 0, s>>>(d->d_seg, d->d_seg + nseg, (int) nseg, sub, B.sub_first);
+                const uint8_t *a_stream = d_stream;
+                const uint32_t *a_begin = d->d_seg, *a_end = d->d_seg + nseg;
+                int a_nseg = (int) nseg;
+                const dec_tables *a_tables = d->d_tables;
+                dec_geom a_g = g;
+                uint32_t a_cap = (uint32_t) cap;
+                void *args[] = { &a_stream, &a_begin, &a_end, &a_nseg, (void *) &sub, &a_tables, &a_g, &dev_scans, &B, &a_cap };
+                if (cudaLaunchCooperativeKernel((const void *) jpeg_sync_kernel, grid, kSyncThreads, args, kTablesSmem, s) != cudaSuccess) {
+                        return -2;
+                }
+                lap("+sync rounds + scan");
+                const unsigned wgrid = (unsigned) ((cap + kHuffThreads - 1) / kHuffThreads);
+                if (full) {
+                        jpeg_sync_write_kernel<true><<<wgrid, kHuffThreads, hsmem, s>>>(d_stream, d->d_seg, d->d_seg + nseg, (int) nseg, sub, d->d_tables, g, d->coef,
+                                                                                       dev_scans, B, (uint32_t) cap);
+                } else {
+                        cudaMemsetAsync(d->coef, 0, (size_t) g.nblocks * 128, s);
+                        jpeg_sync_write_kernel<false><<<wgrid, kHuffThreads, hsmem, s>>>(d_stream, d->d_seg, d->d_seg + nseg, (int) nseg, sub, d->d_tables, g, d->coef,
+                                                                                        dev_scans, B, (uint32_t) cap);
+                }
+                lap("+sync write");
+                d->last_sync_ctr = B.ctr, d->last_sync_scans = g.nscans;
+        } else if (full) {
                 jpeg_decode_huffman_kernel<true><<<hgrid, kHuffThreads, hsmem, s>>>(d_stream, d->d_seg, d->d_seg + nseg, d->d_tables, g, d->coef, dev_scans);
         } else {
                 cudaMemsetAsync(d->coef, 0, (size_t) g.nblocks * 128, s);
