@@ -60,7 +60,8 @@ UGB_API void ugb200_jpeg_encoder_destroy(ugb200_jpeg_encoder *enc);
  * buffer, the capacity the reference gives libgpujpeg at gpujpeg.cpp:355 (noise at quality ~100 only). */
 UGB_API int ugb200_jpeg_encode_device(ugb200_jpeg_encoder *enc, const void *src, long pitch, int width, int height, int codec,
                                       const struct ugb200_jpeg_params *params);
-enum { UGB200_JPEG_CS_NATIVE = 0, UGB200_JPEG_CS_Y601, UGB200_JPEG_CS_Y601FULL, UGB200_JPEG_CS_Y709, UGB200_JPEG_CS_RGB };  /* = gpujpeg_opts::internal_cs */
+enum { UGB200_JPEG_CS_NATIVE = 0, UGB200_JPEG_CS_Y601, UGB200_JPEG_CS_Y601FULL, UGB200_JPEG_CS_Y709, UGB200_JPEG_CS_RGB,  /* = gpujpeg_opts::internal_cs */
+       UGB200_JPEG_CS_AUTO = 5 /* decode only: the colour space the stream declares (ugb200_jpeg_stream_color_space) */ };
 struct ugb200_jpeg_params_ex {
         struct ugb200_jpeg_params base;
         int subsampling;   /* 0 = native for the input (RGB 444, UYVY 422, I420 420), else 444 / 422 / 420 */
@@ -153,6 +154,31 @@ UGB_API int ugb200_jpeg_decoder_expect(ugb200_jpeg_decoder *dec, int width, int 
  * 0 ok, -1 bad arguments, -2 CUDA failure, -3 malformed stream, -4 unsupported stream or output codec. */
 UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *dec, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch,
                                int out_codec, int rshift, int gshift, int bshift);
+
+/* Decode in a colour space.  ugb200_jpeg_decode writes the stream's samples (no colour transform in the codec); its RGB and RGBA output of a YCbCr
+ * stream is that of UltraGrid's line converters, which take every stream as BT.709 limited range.  A JFIF stream (libjpeg, PIL, webcams) holds
+ * full-range BT.601 (T.871), so its colours come out wrong that way.
+ *
+ * ugb200_jpeg_stream_color_space (host only) returns the colour space the stream declares, or < 0 (-1 bad arguments, -3 malformed, -4 unsupported):
+ *   RGB and RGBA streams (Adobe transform 0, component ids 'R' 'G' 'B', four components) -> UGB200_JPEG_CS_RGB, whatever else they carry;
+ *   else a SPIFF APP8: colour space 1 -> Y709, 4 -> Y601, 3 -> Y601FULL, 10 -> RGB, any other code -> -4, a segment too short for the field -> -3;
+ *   else Adobe APP14 transform 1 -> Y601FULL; else JFIF APP0 -> Y601FULL; else (no marker) -> Y709, what UltraGrid assumes for unmarked streams.
+ *
+ * ugb200_jpeg_decode_cs is ugb200_jpeg_decode, except that RGB and RGBA output of a YCbCr stream is converted from `color_space`:
+ *   UGB200_JPEG_CS_NATIVE: the bytes of ugb200_jpeg_decode.
+ *   UGB200_JPEG_CS_Y709 | _Y601 | _Y601FULL: what the stream's YCbCr holds.  R = clamp((y_scale * (Y - o) + r_cr * (Cr - 128)) >> 14, 0, 255), G and B
+ *     likewise (UltraGrid's YCBCR_TO_R/G/B) with the coefficients coeffs_709(8), coeffs_601(8), coeffs_601(0) of UltraGrid's color_space.c, o = 16,
+ *     16, 0, and >> a floor.  Chroma is replicated from its pixel pair (4:2:2) or quad (4:2:0), not interpolated.  RGBA places R, G and B at the
+ *     shifts and sets every other bit (alpha 0xFF).  Y709 RGB output of a 4:2:2 or 4:2:0 stream is the RGB of ugb200_jpeg_decode byte for byte.
+ *   UGB200_JPEG_CS_AUTO: as ugb200_jpeg_stream_color_space resolves it; a stream that declares RGB is not transformed, a refusal is returned.
+ * RGB and four-component streams, and UYVY, I420 and VUYA output, keep the stream's samples in every mode (no YCbCr -> YCbCr matrix conversion).
+ * As in ugb200_jpeg_decode, RGB and RGBA rows of a 4:2:2 / 4:2:0 stream of odd width get whole pixel pairs only (DESIGN.md section 8).
+ * Any other color_space returns -1.  On every error the output buffer is not touched.
+ * Known limitation: this library's encoder writes JFIF APP0 on its UYVY and I420 streams although they hold BT.709 limited-range samples, so
+ * AUTO reads them as Y601FULL; callers that decode this encoder's streams pass Y709 or NATIVE. */
+UGB_API int ugb200_jpeg_stream_color_space(const uint8_t *stream, size_t len);
+UGB_API int ugb200_jpeg_decode_cs(ugb200_jpeg_decoder *dec, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch,
+                                  int out_codec, int rshift, int gshift, int bshift, int color_space);
 
 #ifdef __cplusplus
 }

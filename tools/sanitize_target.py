@@ -134,6 +134,22 @@ if ONLY != "staged":
                 n += 1
         dec3.close()
     os.environ.pop("UGB200_JPEG_SYNC", None)
+# JPEG decoder, fused IDCT + chroma replication + packing kernel (4:2:2 and 4:2:0) and the 4:4:4 colour-space kernel: odd and even sizes, tight
+# device buffers and a pitch wider than the row, UYVY / RGB / RGBA with shifts (8, 16, 0), every colour space
+if ONLY != "staged":
+    dec4 = api.JpegDecoder()
+    for ss, w, h in ((1, 333, 211), (2, 333, 211), (2, 64, 32), (0, 37, 19)):
+        b = io.BytesIO()
+        Image.fromarray(natural_rgb(w, h, 6)).save(b, "JPEG", quality=90, subsampling=ss)
+        s = b.getvalue()
+        for out_c, bpp in ((2, 2), (12, 3), (1, 4)):
+            ls = vc_get_linesize(w, out_c)
+            for pitch in (ls, ls + 40):
+                for cs in ((None,) if out_c == 2 else (None, "native", "Y709", "Y601", "Y601full", "auto")):
+                    out = torch.empty(pitch * h, dtype=torch.uint8, device="cuda")
+                    dec4.decode(s, out_c, shifts=(8, 16, 0) if out_c == 1 else (0, 8, 16), device=True, pitch=pitch, out=out, color_space=cs)
+                    n += 1
+    dec4.close()
 # LDGM FEC: encode from host (packets of 4-, 8- and 16-byte words) and from a device frame at offsets 4 and 1 into a tight device buffer;
 # decode with losses peeling can repair (several levels) and with losses it cannot
 import ldgm_cases as lc

@@ -368,8 +368,10 @@ class JpegDecoder:
         _check(_L.ugb200_jpeg_decoder_last_sync(self._h, ctypes.byref(st)), "ugb200_jpeg_decoder_last_sync")
         return {"scans": st.scans, "subsequences": st.subsequences, "rounds": st.rounds}
 
-    def decode(self, stream, out_codec, shifts=(0, 8, 16), device=False, pitch=0, out=None, sync=True):
-        """bytes -> numpy array (host) or CUDA tensor (device=True) holding height rows of vc_get_linesize(width, out_codec) bytes"""
+    def decode(self, stream, out_codec, shifts=(0, 8, 16), device=False, pitch=0, out=None, sync=True, color_space=None):
+        """bytes -> numpy array (host) or CUDA tensor (device=True) holding height rows of vc_get_linesize(width, out_codec) bytes.
+        ``color_space`` None: ugb200_jpeg_decode (the stream's samples, RGB / RGBA through UltraGrid's line converters); else one of
+        JPEG_CS (``"native"``, ``"Y709"``, ``"Y601"``, ``"Y601full"``, ``"auto"``) or its value: ugb200_jpeg_decode_cs"""
         info = jpeg_image_info(stream)
         ls = pitch or vc_get_linesize(info.width, out_codec)
         nbytes = ls * info.height
@@ -381,14 +383,32 @@ class JpegDecoder:
                 out = torch.zeros(nbytes, dtype=torch.uint8, device="cuda")
             elif out.numel() * out.element_size() < nbytes:
                 raise ValueError(f"out holds {out.numel() * out.element_size()} bytes, the stream decodes to {nbytes}")
-            _check(_L.ugb200_jpeg_decode(self._h, buf, len(stream), _ptr(out), 1, ls, int(out_codec), *shifts), "ugb200_jpeg_decode")
+            self._decode(buf, len(stream), _ptr(out), 1, ls, out_codec, shifts, color_space)
             if sync:
                 self._stream.synchronize()
             return out
         import numpy as np
         out = np.zeros(nbytes, dtype=np.uint8)
-        _check(_L.ugb200_jpeg_decode(self._h, buf, len(stream), ctypes.c_void_p(out.ctypes.data), 0, ls, int(out_codec), *shifts), "ugb200_jpeg_decode")
+        self._decode(buf, len(stream), ctypes.c_void_p(out.ctypes.data), 0, ls, out_codec, shifts, color_space)
         return out
+
+    def _decode(self, buf, n, dst, is_device, pitch, out_codec, shifts, color_space):
+        if color_space is None:
+            _check(_L.ugb200_jpeg_decode(self._h, buf, n, dst, is_device, pitch, int(out_codec), *shifts), "ugb200_jpeg_decode")
+        else:
+            cs = JPEG_CS[color_space] if isinstance(color_space, str) else int(color_space)
+            _check(_L.ugb200_jpeg_decode_cs(self._h, buf, n, dst, is_device, pitch, int(out_codec), *shifts, cs), "ugb200_jpeg_decode_cs")
+
+
+# UGB200_JPEG_CS_* of include/ugb200_jpeg.h
+JPEG_CS = {"native": 0, "Y601": 1, "Y601full": 2, "Y709": 3, "RGB": 4, "auto": 5}
+
+
+def jpeg_stream_color_space(stream):
+    """ugb200_jpeg_stream_color_space: the colour space the stream declares, as a key of JPEG_CS (raises on a refusal)"""
+    rc = _L.ugb200_jpeg_stream_color_space(_bytes_ptr(stream), len(stream))
+    _check(min(rc, 0), "ugb200_jpeg_stream_color_space")
+    return {v: k for k, v in JPEG_CS.items()}[rc]
 
 
 class LdgmCoder:

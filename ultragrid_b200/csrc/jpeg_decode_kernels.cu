@@ -14,9 +14,12 @@
 //                           coefficients as K1 for any bytes (both use jpeg_huffman_step.cuh; see the comment above jpeg_sync_kernel)
 //   K2     jpeg_idct_kernel one thread per 8x8 block: dequantise, float AAN inverse DCT (fixed operation order = bit-exact with
 //                           oracle/jpeg_decode_oracle.c), level shift, clamp, 8 x 8-byte stores into the component plane
-//   pack   the component planes go through the from_planar kernels that already exist (planar_conv_kernels.cu):
-//                           4:2:2 -> UYVY (yuv422p_to_uyvy), 4:2:0 -> UYVY (yuv420p_to_uyvy), 4:4:4 YCbCr -> VUYA (yuv444p_to_vuya),
-//                           RGB -> RGB (rgbpXX_to_rgb), then ugb200_pixfmt_convert when another output codec was asked for.
+//   K2'    jpeg_idct_packed_kernel  instead of K2 for 4:2:2 and 4:2:0 YCbCr: the IDCT of an MCU row's blocks into a shared tile, chroma replicated
+//                           from its pair or quad, and the UYVY words stored as UYVY or handed to a line converter functor (yuv_rgb_conv.cuh):
+//                           UltraGrid's UYVY -> RGB / RGBA, or the integer YCbCr -> RGB of a colour space (ugb200_jpeg_decode_cs); no planes
+//   pack   the component planes of K2 go through the from_planar kernels that already exist (planar_conv_kernels.cu): 4:4:4 YCbCr -> VUYA
+//                           (yuv444p_to_vuya), RGB -> RGB (rgbpXX_to_rgb), R G B A (gbrap_to_rgba); then ugb200_pixfmt_convert when another
+//                           output codec was asked for (also from K2's UYVY to VUYA / I420).  4:4:4 YCbCr in a colour space: jpeg_planes_cs_kernel.
 // Restart intervals are the unit of parallelism of K1; K1' does not depend on them.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -33,12 +36,14 @@
 #include <cstdio>
 #include <new>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/ugb200.h"
 #include "../../include/ugb200_jpeg.h"
 #include "jpeg_marker_bounds.cuh"
 #include "jpeg_huffman_step.cuh"
+#include "yuv_rgb_conv.cuh"
 #include "../../include/cuda_wrapper.h"
 
 #include <cooperative_groups.h>
@@ -580,26 +585,66 @@ __global__ void __launch_bounds__(128) jpeg_idct_kernel(const int16_t *__restric
         }
 }
 
-/// 4:2:2 streams: IDCT and UYVY packing in one kernel.  CTA = 32 MCUs x (Y0, Y1, Cb, Cr), warp k = block kind k (component-uniform
-/// dequantisation), lane = MCU.  The 8 x 8 samples of each block go to a shared tile as 8-byte rows; then the 8 KB tile leaves as 512
-/// 16-byte UYVY pieces, consecutive pieces consecutive in memory.  Same arithmetic as jpeg_idct_kernel.
-__global__ void __launch_bounds__(128) jpeg_idct_uyvy_kernel(const int16_t *__restrict__ coef, const dec_tables *__restrict__ tables, dec_geom g,
-                                                             uint8_t *__restrict__ out, long pitch, bool vec_ok)
+/// UYVY output: the pixel pair words as they are, 16 bytes (8 pixels) per piece
+struct epi_uyvy {
+        static constexpr int PX = 8, OUT = 16, BPP = 2;
+        static __device__ __forceinline__ void run(const uint32_t *w, uint32_t *o, const conv_params &) { o[0] = w[0], o[1] = w[1], o[2] = w[2], o[3] = w[3]; }
+};
+/// RGB / RGBA output: a line converter functor (yuv_rgb_conv.cuh) applied to the UYVY words of 16 pixels, as ugb200_pixfmt_convert would apply it
+/// to the UYVY frame
+template <class C>
+struct epi_conv {
+        static constexpr int PX = 16, OUT = C::OUT * 32 / C::IN, BPP = OUT / 16;
+        static __device__ __forceinline__ void run(const uint32_t *w, uint32_t *o, const conv_params &p)
+        {
+#pragma unroll
+                for (int k = 0; k < 32 / C::IN; ++k) {
+                        C::run(w + k * (C::IN / 4), o + k * (C::OUT / 4), p, row_ctx{});
+                }
+        }
+};
+using epi_rgb = epi_conv<conv_yuv422_rgb<1, 3, 0, 2>>;  // vc_copylineUYVYtoRGB = BT.709 limited range
+using epi_rgba = epi_conv<conv_uyvy_rgba>;             // vc_copylineUYVYtoRGBA
+template <class CS>
+using epi_cs_rgb = epi_conv<conv_yuv422_rgb<1, 3, 0, 2, CS>>;
+template <class CS>
+using epi_cs_rgba = epi_conv<conv_yuv422_rgb<1, 3, 0, 2, CS, true>>;
+
+/// the UYVY words of 8 pixels: 8 luma samples, the 4 Cb and 4 Cr samples of their pairs
+__device__ __forceinline__ void uyvy_words(uint2 Y, uint32_t C, uint32_t R, uint32_t *w)
 {
+        w[0] = __byte_perm(__byte_perm(C, R, 0x0040), Y.x, 0x5140), w[1] = __byte_perm(__byte_perm(C, R, 0x0051), Y.x, 0x7160);
+        w[2] = __byte_perm(__byte_perm(C, R, 0x0062), Y.y, 0x5140), w[3] = __byte_perm(__byte_perm(C, R, 0x0073), Y.y, 0x7160);
+}
+
+/// 4:2:2 (V = 1) and 4:2:0 (V = 2) YCbCr streams: IDCT, chroma replication and packing in one kernel, no component planes.  CTA = 32 MCUs of one
+/// MCU row x the MCU's blocks (4:2:2: Y0 Y1 Cb Cr; 4:2:0: Y0 Y1 Y2 Y3 Cb Cr), warp k = block kind k (component-uniform dequantisation), lane = MCU.
+/// The 8 x 8 samples of each block go to a shared tile as 8-byte rows.  The tile then leaves as UYVY words, the chroma of a pair row shared by both luma
+/// rows of a 4:2:0 MCU (what yuv420p_to_uyvy does), through the epilogue E: as UYVY in 16-byte pieces, consecutive threads consecutive in memory; or
+/// converted to RGB / RGBA, 16 pixels per thread, staged per warp in shared memory so that each warp stores its row's run as consecutive 16-byte
+/// pieces.  Same IDCT arithmetic as jpeg_idct_kernel.  A row holds ((w + 1) / 2) * 4 bytes of UYVY (the last pair of an odd width takes the padded
+/// plane's luma) but only whole pixel pairs of RGB / RGBA (the line converters' out_len), and rows but the last stop at the pitch, as there.
+template <int V, class E>
+__global__ void __launch_bounds__(32 * (2 * V + 2)) jpeg_idct_packed_kernel(const int16_t *__restrict__ coef, const dec_tables *__restrict__ tables, dec_geom g,
+                                                                            uint8_t *__restrict__ out, long pitch, bool vec_ok, conv_params p)
+{
+        constexpr int NB = 2 * V + 2, NT = 32 * NB, ROWS = 8 * V, PPR = 32 * 16 / E::PX;  // blocks per MCU, threads, pixel rows, pieces per row
+        constexpr bool STAGED = E::PX == 16;
         __shared__ float s_m[4][64];
-        __shared__ uint2 s_tile[4][8][32];
+        __shared__ uint2 s_tile[NB][8][32];
+        __shared__ uint4 s_out[STAGED ? NB : 1][STAGED ? 32 * E::OUT / 16 : 1];
         const int tid = threadIdx.x;
-        for (int i = tid; i < 256; i += blockDim.x) {
+        for (int i = tid; i < 256; i += NT) {
                 s_m[i >> 6][i & 63] = tables->m[i >> 6][i & 63];
         }
         __syncthreads();
-        const int mcux = g.c[1].bw, nmcu = mcux * g.c[1].bh;
-        const int k = tid >> 5, lane = tid & 31, m0 = blockIdx.x * 32, m = m0 + lane;
-        if (m < nmcu) {
-                const int mx = m % mcux, my = m / mcux;
-                const dec_comp &c = g.c[k < 2 ? 0 : k - 1];
-                const int X = k < 2 ? 2 * mx + k : mx;
-                const long b = (long) c.blk_off + (long) my * c.bw + X;
+        const int mcux = g.c[1].bw, my = blockIdx.y, mx0 = blockIdx.x * 32;
+        const int k = tid >> 5, lane = tid & 31, mx = mx0 + lane;
+        if (mx < mcux) {
+                const int ci = k < 2 * V ? 0 : k - 2 * V + 1;
+                const dec_comp &c = g.c[ci];
+                const int X = ci == 0 ? 2 * mx + (k & 1) : mx, Y = ci == 0 ? V * my + (k >> 1) : my;
+                const long b = (long) c.blk_off + (long) Y * c.bw + X;
                 const float *mq = s_m[c.tq];
                 float f[64];
                 const uint4 *src = (const uint4 *) (coef + b * 64);
@@ -631,31 +676,89 @@ __global__ void __launch_bounds__(128) jpeg_idct_uyvy_kernel(const int16_t *__re
                 }
         }
         __syncthreads();
-        const int row_bytes = ((g.w + 1) / 2) * 4;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-                const int cidx = tid + 128 * i, row = cidx >> 6, within = cidx & 63, mcu = within >> 1, half = within & 1;
-                const int mm = m0 + mcu;
-                if (mm >= nmcu) {
-                        continue;
+        const int row_full = E::BPP == 2 ? ((g.w + 1) / 2) * 4 : (g.w / 2) * 2 * E::BPP;
+        for (int cidx = tid; cidx < ROWS * PPR; cidx += NT) {
+                const int row = cidx / PPR, piece = cidx % PPR, mcu = piece / (16 / E::PX), half = piece % (16 / E::PX);
+                const int y = my * ROWS + row;
+                if (y >= g.h) {  // uniform over the warp
+                        break;
                 }
-                const int mx = mm % mcux, y = (mm / mcux) * 8 + row, xoff = mx * 32 + half * 16;
-                if (y >= g.h || xoff >= row_bytes) {
-                        continue;
-                }
-                const uint2 Y = s_tile[half][row][mcu], CB = s_tile[2][row][mcu], CR = s_tile[3][row][mcu];
-                const uint32_t C = half ? CB.y : CB.x, R = half ? CR.y : CR.x;
-                const uint32_t w0 = __byte_perm(__byte_perm(C, R, 0x0040), Y.x, 0x5140), w1 = __byte_perm(__byte_perm(C, R, 0x0051), Y.x, 0x7160);
-                const uint32_t w2 = __byte_perm(__byte_perm(C, R, 0x0062), Y.y, 0x5140), w3 = __byte_perm(__byte_perm(C, R, 0x0073), Y.y, 0x7160);
-                uint8_t *d = out + (long) y * pitch + xoff;
-                if (vec_ok && xoff + 16 <= row_bytes) {
-                        *(uint4 *) d = make_uint4(w0, w1, w2, w3);
+                const int lim = E::BPP == 2 || y == g.h - 1 || row_full <= pitch ? row_full : (int) pitch;
+                const int cb = 2 * V, crow = V == 2 ? row >> 1 : row, yb = V == 2 ? 2 * (row >> 3) : 0, yrow = row & 7;
+                const uint2 CB = s_tile[cb][crow][mcu], CR = s_tile[cb + 1][crow][mcu];
+                uint32_t w[E::PX / 2], o[E::OUT / 4];
+                if (E::PX == 8) {
+                        uyvy_words(s_tile[yb + half][yrow][mcu], half ? CB.y : CB.x, half ? CR.y : CR.x, w);
                 } else {
-                        const uint32_t w[4] = { w0, w1, w2, w3 };
-                        for (int bq = 0; bq < 16 && xoff + bq < row_bytes; ++bq) {
-                                d[bq] = (uint8_t) (w[bq >> 2] >> (8 * (bq & 3)));
-                        }
+                        uyvy_words(s_tile[yb][yrow][mcu], CB.x, CR.x, w);
+                        uyvy_words(s_tile[yb + 1][yrow][mcu], CB.y, CR.y, w + 4);
                 }
+                E::run(w, o, p);
+                uint8_t *d = out + (long) y * pitch;
+                if constexpr (!STAGED) {
+                        const int xoff = (mx0 + mcu) * 32 + half * 16;
+                        if (mx0 + mcu >= mcux || xoff >= lim) {
+                                continue;
+                        }
+                        if (vec_ok && xoff + 16 <= lim) {
+                                *(uint4 *) (d + xoff) = make_uint4(o[0], o[1], o[2], o[3]);
+                        } else {
+                                for (int bq = 0; bq < 16 && xoff + bq < lim; ++bq) {
+                                        d[xoff + bq] = (uint8_t) (o[bq >> 2] >> (8 * (bq & 3)));
+                                }
+                        }
+                } else {  // the warp holds one row's 32 pieces: stage them, then store the run as consecutive 16-byte pieces
+                        constexpr int NQ = E::OUT / 16;
+                        uint4 *sw = s_out[k];
+#pragma unroll
+                        for (int q = 0; q < NQ; ++q) {
+                                sw[lane * NQ + q] = make_uint4(o[4 * q], o[4 * q + 1], o[4 * q + 2], o[4 * q + 3]);
+                        }
+                        __syncwarp();
+                        const int x0 = mx0 * 16 * E::BPP, run = min(lim - x0, 32 * E::OUT);
+#pragma unroll
+                        for (int q = 0; q < NQ; ++q) {
+                                const int off = (q * 32 + lane) * 16;
+                                if (off >= run) {
+                                        continue;
+                                }
+                                const uint4 v = sw[q * 32 + lane];
+                                if (vec_ok && off + 16 <= run) {
+                                        *(uint4 *) (d + x0 + off) = v;
+                                } else {
+                                        const uint32_t vw[4] = { v.x, v.y, v.z, v.w };
+                                        for (int bq = 0; bq < 16 && off + bq < run; ++bq) {
+                                                d[x0 + off + bq] = (uint8_t) (vw[bq >> 2] >> (8 * (bq & 3)));
+                                        }
+                                }
+                        }
+                        __syncwarp();
+                }
+        }
+}
+
+/// 4:4:4 YCbCr streams to RGB / RGBA in a colour space: one thread per pixel over the component planes of jpeg_idct_kernel (same formula as
+/// conv_yuv422_rgb<..., CS>, in integers)
+template <class CS, bool RGBA>
+__global__ void __launch_bounds__(256) jpeg_planes_cs_kernel(const uint8_t *__restrict__ planes, dec_geom g, uint8_t *__restrict__ out, long pitch, conv_params p)
+{
+        const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+        if (x >= g.w) {
+                return;
+        }
+        constexpr color_coeffs c = CS::coeffs();
+        const long ls = (long) g.c[0].bw * 8;  // 1x1 sampling: the three planes have the same line size
+        const int Y = planes[g.c[0].plane_off + y * ls + x] - CS::y_off, cb = planes[g.c[1].plane_off + y * ls + x] - 128,
+                  cr = planes[g.c[2].plane_off + y * ls + x] - 128;
+        const int ys = c.y_scale * Y;
+        const uint32_t r = (uint32_t) min(max((ys + c.r_cr * cr) >> COMP_BASE, 0), 255), gg = (uint32_t) min(max((ys + c.g_cb * cb + c.g_cr * cr) >> COMP_BASE, 0), 255),
+                       b = (uint32_t) min(max((ys + c.b_cb * cb) >> COMP_BASE, 0), 255);
+        uint8_t *d = out + (long) y * pitch;
+        if (RGBA) {
+                const uint32_t v = (0xFFFFFFFFu ^ (0xFFu << p.rshift) ^ (0xFFu << p.gshift) ^ (0xFFu << p.bshift)) | r << p.rshift | gg << p.gshift | b << p.bshift;
+                d[4 * x] = (uint8_t) v, d[4 * x + 1] = (uint8_t) (v >> 8), d[4 * x + 2] = (uint8_t) (v >> 16), d[4 * x + 3] = (uint8_t) (v >> 24);
+        } else {
+                d[3 * x] = (uint8_t) r, d[3 * x + 1] = (uint8_t) gg, d[3 * x + 2] = (uint8_t) b;
         }
 }
 
@@ -995,6 +1098,8 @@ struct huff_defs {  // the current DHT definition of each table id, built into a
 struct parsed {
         dec_geom g{};
         int adobe = -1, comp_id[4] = { 0, 0, 0, 0 };
+        int spiff = -1;  // colour space field of the first SPIFF APP8, -2 when that segment is too short to hold it
+        bool jfif = false;
         bool have_sof = false, have_q[4] = { false, false, false, false };
         huff_defs hd;
         uint8_t q[4][64];
@@ -1213,6 +1318,10 @@ int parse_stream(const uint8_t *s, size_t len, parsed &P, dec_tables *T, bool fu
                         g.ri = be16(d);
                 } else if (mk == 0xEE && L >= 14 && memcmp(d, "Adobe", 5) == 0) {
                         P.adobe = d[11];
+                } else if (mk == 0xE8 && L >= 8 && memcmp(d, "SPIFF", 6) == 0 && P.spiff == -1) {
+                        P.spiff = L >= 21 ? d[18] : -2;  // identifier 6, version 2, profile 1, components 1, height 4, width 4, colour space 1
+                } else if (mk == 0xE0 && L >= 7 && memcmp(d, "JFIF", 5) == 0) {
+                        P.jfif = true;
                 } else if (mk == 0xDA) {
                         if (!P.have_sof || g.nscans >= g.ncomp) {
                                 return -3;
@@ -1340,6 +1449,29 @@ int native_codec(const parsed &P)
         return rgb ? UGB_RGB : UGB_VUYA;
 }
 
+/// the colour space the stream declares (ugb200_jpeg_stream_color_space): UGB200_JPEG_CS_*, or -3 / -4
+int declared_color_space(const parsed &P)
+{
+        const int nc = native_codec(P);
+        if (nc == UGB_RGB || nc == UGB_RGBA) {
+                return UGB200_JPEG_CS_RGB;
+        }
+        if (P.spiff != -1) {  // SPIFF colour space codes (ITU-T T.84 Annex F)
+                switch (P.spiff) {
+                case -2: return -3;
+                case 1: return UGB200_JPEG_CS_Y709;
+                case 3: return UGB200_JPEG_CS_Y601FULL;
+                case 4: return UGB200_JPEG_CS_Y601;
+                case 10: return UGB200_JPEG_CS_RGB;
+                default: return -4;
+                }
+        }
+        if (P.adobe == 1 || P.jfif) {  // Adobe APP14 transform 1, JFIF (T.871): full-range BT.601
+                return UGB200_JPEG_CS_Y601FULL;
+        }
+        return UGB200_JPEG_CS_Y709;  // no marker: what UltraGrid tells GPUJPEG to assume (src/video_decompress/gpujpeg.c:103-112)
+}
+
 }  // namespace
 
 extern "C" {
@@ -1359,6 +1491,16 @@ UGB_API int ugb200_jpeg_get_image_info(const uint8_t *stream, size_t len, struct
         info->adobe_transform = P.adobe, info->restart_interval = P.g.ri;
         info->native_codec = native_codec(P);
         return 0;
+}
+
+UGB_API int ugb200_jpeg_stream_color_space(const uint8_t *stream, size_t len)
+{
+        if (!stream) {
+                return -1;
+        }
+        parsed P;
+        const int rc = parse_stream(stream, len, P, nullptr, false);
+        return rc != 0 ? rc : declared_color_space(P);
 }
 
 UGB_API long ugb200_jpeg_debug_segments(const uint8_t *stream, size_t len, uint32_t *begin, uint32_t *end, long cap)
@@ -1493,8 +1635,9 @@ UGB_API int ugb200_jpeg_decoder_expect(ugb200_jpeg_decoder *d, int width, int he
         return 0;
 }
 
-UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec,
-                               int rshift, int gshift, int bshift)
+/// ugb200_jpeg_decode and ugb200_jpeg_decode_cs: color_space is one of NATIVE, Y601, Y601FULL, Y709, AUTO
+static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec, int rshift, int gshift,
+                  int bshift, int color_space)
 {
         const long dst_pitch_arg = dst_pitch;
         if (!d || !stream || !dst || len > 0xFFFFFFF0u) {
@@ -1638,6 +1781,13 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
         const int native = alpha && out_codec != UGB_RGBA ? UGB_RGB : stream_codec;
         const long npitch = native == UGB_UYVY ? (long) ((g.w + 1) / 2) * 4 : native == UGB_RGB ? (long) g.w * 3 : (long) g.w * 4;
         const long opitch = out_codec == UGB_UYVY ? (long) ((g.w + 1) / 2) * 4 : out_codec == UGB_RGB ? (long) g.w * 3 : (long) g.w * 4;
+        // RGB and RGBA output of a YCbCr stream in a colour space (ugb200_jpeg_decode_cs); AUTO takes the stream's, and one that declares RGB is not transformed
+        const int cs = color_space == UGB200_JPEG_CS_AUTO ? declared_color_space(P) : color_space;
+        if (cs < 0) {
+                return cs;
+        }
+        const int conv_cs = (native == UGB_UYVY || native == UGB_VUYA) && (out_codec == UGB_RGB || out_codec == UGB_RGBA) && cs != UGB200_JPEG_CS_RGB ? cs
+                                                                                                                                               : UGB200_JPEG_CS_NATIVE;
         if (dst_pitch == 0) {
                 dst_pitch = opitch;
         }
@@ -1681,7 +1831,7 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
                         lap("verdict");
                         if (*d->h_flag != 0) {
                                 d->host_once = true;
-                                return ugb200_jpeg_decode(d, stream, len, dst, dst_is_device, dst_pitch_arg, out_codec, rshift, gshift, bshift);
+                                return decode(d, stream, len, dst, dst_is_device, dst_pitch_arg, out_codec, rshift, gshift, bshift, color_space);
                         }
                 } else {
                         jpeg_marker_segments_kernel<<<(unsigned) ((nseg + 255) / 256), 256, 0, s>>>(d->d_marks, meta, (uint32_t) scan_data, (uint32_t) len, (int) nseg, d->d_seg,
@@ -1781,46 +1931,99 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
         H.consumed_pending = true;
         const bool direct = native == out_codec && dst_is_device && !reshift;
         uint8_t *nat = direct ? (uint8_t *) dst : d->native;
-        const bool fused_uyvy = native == UGB_UYVY && g.c[0].v == 1;  // 4:2:2: IDCT and packing in one kernel, no component planes
-        if (fused_uyvy) {
-                const long np = direct ? dst_pitch : npitch;
-                jpeg_idct_uyvy_kernel<<<(g.c[1].bw * g.c[1].bh + 31) / 32, 128, 0, s>>>(d->coef, d->d_tables, g, nat, np, !(15 & (size_t) nat) && !(np & 15));
+        // the caller's RGB / RGBA in a colour space, or any output of the fused kernel: into dst when it is on the device, else into staging and across
+        const bool fused = native == UGB_UYVY, to_out = conv_cs != UGB200_JPEG_CS_NATIVE || (fused && (out_codec == UGB_RGB || out_codec == UGB_RGBA));
+        if (to_out && !dst_is_device && !dgrow(d->staging, d->staging_cap, (size_t) opitch * g.h + 64)) {
+                return -2;
+        }
+        uint8_t *const conv = dst_is_device ? (uint8_t *) dst : d->staging;
+        const long cpitch = dst_is_device ? dst_pitch : opitch;
+        const conv_params cp = { rshift, gshift, bshift, 0 };
+        if (fused) {  // 4:2:2 and 4:2:0: IDCT, chroma replication and packing (or conversion) in one kernel, no component planes
+                const bool uyvy_out = !to_out;
+                uint8_t *o = uyvy_out ? nat : conv;
+                const long op = uyvy_out ? (direct ? dst_pitch : npitch) : cpitch;
+                const dim3 grid((unsigned) ((g.c[1].bw + 31) / 32), (unsigned) g.c[1].bh);
+                const bool vec = !(15 & (size_t) o) && !(op & 15);
+                const int kind = uyvy_out ? 0 : out_codec == UGB_RGB ? (conv_cs == UGB200_JPEG_CS_NATIVE ? UGB200_JPEG_CS_Y709 : conv_cs) : 4 + conv_cs;
+                auto launch = [&](auto v) {
+                        constexpr int V = decltype(v)::value;
+                        switch (kind) {
+                        case 0: jpeg_idct_packed_kernel<V, epi_uyvy><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp); break;
+                        case UGB200_JPEG_CS_Y709: jpeg_idct_packed_kernel<V, epi_rgb><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp); break;
+                        case UGB200_JPEG_CS_Y601: jpeg_idct_packed_kernel<V, epi_cs_rgb<ycbcr_601>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp); break;
+                        case UGB200_JPEG_CS_Y601FULL:
+                                jpeg_idct_packed_kernel<V, epi_cs_rgb<ycbcr_601_full>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp);
+                                break;
+                        case 4 + UGB200_JPEG_CS_NATIVE: jpeg_idct_packed_kernel<V, epi_rgba><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp); break;
+                        case 4 + UGB200_JPEG_CS_Y709:
+                                jpeg_idct_packed_kernel<V, epi_cs_rgba<ycbcr_709>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp);
+                                break;
+                        case 4 + UGB200_JPEG_CS_Y601:
+                                jpeg_idct_packed_kernel<V, epi_cs_rgba<ycbcr_601>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp);
+                                break;
+                        default:
+                                jpeg_idct_packed_kernel<V, epi_cs_rgba<ycbcr_601_full>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp);
+                                break;
+                        }
+                };
+                if (g.c[0].v == 2) {
+                        launch(std::integral_constant<int, 2>());
+                } else {
+                        launch(std::integral_constant<int, 1>());
+                }
         } else {
                 jpeg_idct_kernel<<<(g.nblocks + 127) / 128, 128, 0, s>>>(d->coef, d->d_tables, g, d->planes);
+                if (to_out) {  // 4:4:4 YCbCr in a colour space: per pixel over the planes
+                        const dim3 grid((unsigned) ((g.w + 255) / 256), (unsigned) g.h);
+                        const bool rgba = out_codec == UGB_RGBA;
+                        if (conv_cs == UGB200_JPEG_CS_Y709) {
+                                rgba ? jpeg_planes_cs_kernel<ycbcr_709, true><<<grid, 256, 0, s>>>(d->planes, g, conv, cpitch, cp)
+                                     : jpeg_planes_cs_kernel<ycbcr_709, false><<<grid, 256, 0, s>>>(d->planes, g, conv, cpitch, cp);
+                        } else if (conv_cs == UGB200_JPEG_CS_Y601) {
+                                rgba ? jpeg_planes_cs_kernel<ycbcr_601, true><<<grid, 256, 0, s>>>(d->planes, g, conv, cpitch, cp)
+                                     : jpeg_planes_cs_kernel<ycbcr_601, false><<<grid, 256, 0, s>>>(d->planes, g, conv, cpitch, cp);
+                        } else {
+                                rgba ? jpeg_planes_cs_kernel<ycbcr_601_full, true><<<grid, 256, 0, s>>>(d->planes, g, conv, cpitch, cp)
+                                     : jpeg_planes_cs_kernel<ycbcr_601_full, false><<<grid, 256, 0, s>>>(d->planes, g, conv, cpitch, cp);
+                        }
+                }
         }
         if (cudaGetLastError() != cudaSuccess) {
                 return -2;
         }
         lap("kernels queued");
         lap("+huffman + idct");
-        // component planes -> the stream's native packed format
-        struct ugb200_from_planar_data fp;
-        memset(&fp, 0, sizeof fp);
-        fp.width = native == UGB_UYVY ? (g.w + 1) & ~1 : g.w;  // the padded planes hold the second luma of an odd last pixel pair
-        fp.height = g.h, fp.out_data = nat, fp.out_pitch = (unsigned) (direct ? dst_pitch : npitch);
-        for (int i = 0; i < 3; ++i) {
-                fp.in_data[i] = d->planes + g.c[i].plane_off, fp.in_linesize[i] = (unsigned) (g.c[i].bw * 8);
-        }
-        fp.in_depth = 8;
-        if (alpha) {  // planes in G, B, R, A order (from_planar.c:335-366); all four have the same line size
-                for (int i = 0; i < 4; ++i) {
-                        const dec_comp &c = g.c[i == 3 ? 3 : (i + 1) % 3];
-                        fp.in_data[i] = d->planes + c.plane_off, fp.in_linesize[i] = (unsigned) (c.bw * 8);
+        if (to_out) {
+                if (dst_is_device) {
+                        return 0;
                 }
+                return cudaMemcpy2DAsync(dst, dst_pitch, conv, cpitch, opitch, g.h, cudaMemcpyDeviceToHost, s) == cudaSuccess && cudaStreamSynchronize(s) == cudaSuccess ? 0 : -2;
         }
-        if (fused_uyvy) {
-                rc = 0;
-        } else if (alpha) {
-                rc = native == UGB_RGBA ? ugb200_gbrap_to_rgba(&fp, s) : ugb200_gbrap_to_rgb(&fp, s);
-        } else if (native == UGB_UYVY) {
-                rc = g.c[0].v == 2 ? ugb200_yuv420p_to_uyvy(&fp, s) : ugb200_yuv422p_to_uyvy(&fp, s);
-        } else if (native == UGB_RGB) {
-                rc = ugb200_rgbpXX_to_rgb(&fp, s);
-        } else {
-                rc = ugb200_yuv444p_to_vuya(&fp, s);
-        }
-        if (rc != 0) {
-                return rc;
+        if (!fused) {  // component planes -> the stream's native packed format
+                struct ugb200_from_planar_data fp;
+                memset(&fp, 0, sizeof fp);
+                fp.width = g.w, fp.height = g.h, fp.out_data = nat, fp.out_pitch = (unsigned) (direct ? dst_pitch : npitch);
+                for (int i = 0; i < 3; ++i) {
+                        fp.in_data[i] = d->planes + g.c[i].plane_off, fp.in_linesize[i] = (unsigned) (g.c[i].bw * 8);
+                }
+                fp.in_depth = 8;
+                if (alpha) {  // planes in G, B, R, A order (from_planar.c:335-366); all four have the same line size
+                        for (int i = 0; i < 4; ++i) {
+                                const dec_comp &c = g.c[i == 3 ? 3 : (i + 1) % 3];
+                                fp.in_data[i] = d->planes + c.plane_off, fp.in_linesize[i] = (unsigned) (c.bw * 8);
+                        }
+                }
+                if (alpha) {
+                        rc = native == UGB_RGBA ? ugb200_gbrap_to_rgba(&fp, s) : ugb200_gbrap_to_rgb(&fp, s);
+                } else if (native == UGB_RGB) {
+                        rc = ugb200_rgbpXX_to_rgb(&fp, s);
+                } else {
+                        rc = ugb200_yuv444p_to_vuya(&fp, s);
+                }
+                if (rc != 0) {
+                        return rc;
+                }
         }
         if (direct) {
                 return 0;
@@ -1889,6 +2092,22 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, si
                 return -2;
         }
         return 0;
+}
+
+UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec,
+                               int rshift, int gshift, int bshift)
+{
+        return decode(d, stream, len, dst, dst_is_device, dst_pitch, out_codec, rshift, gshift, bshift, UGB200_JPEG_CS_NATIVE);
+}
+
+UGB_API int ugb200_jpeg_decode_cs(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec,
+                                  int rshift, int gshift, int bshift, int color_space)
+{
+        if (color_space != UGB200_JPEG_CS_NATIVE && color_space != UGB200_JPEG_CS_Y601 && color_space != UGB200_JPEG_CS_Y601FULL &&
+            color_space != UGB200_JPEG_CS_Y709 && color_space != UGB200_JPEG_CS_AUTO) {
+                return -1;
+        }
+        return decode(d, stream, len, dst, dst_is_device, dst_pitch, out_codec, rshift, gshift, bshift, color_space);
 }
 
 }  // extern "C"

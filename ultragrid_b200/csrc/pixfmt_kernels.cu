@@ -13,20 +13,9 @@
 #include "../../include/ugb200.h"
 #include "color_space.h"
 #include "f32x2.cuh"
+#include "yuv_rgb_conv.cuh"
 
 namespace ugb {
-
-struct conv_params {
-        int rshift, gshift, bshift;
-        int aux;  // converter-specific, computed on the host from dst_len (see conv_rgba_rgb)
-};
-/// where a chunk sits, for the rare converter whose result depends on more than its own chunk
-struct row_ctx {
-        const uint8_t *src;  // buffer start
-        long row_abs;        // byte offset of this row in src
-        long src_total;      // readable bytes
-        int cx;              // chunk index within the row
-};
 
 // byte k (compile-time) of a packed word array
 template <int K>
@@ -75,88 +64,6 @@ struct conv_yuyv_uyvy {
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                         out[i] = __byte_perm(in[i], 0, 0x2301);
-                }
-        }
-};
-
-/// copylineYUVtoRGB (pixfmt_conv.c:1065-1094) via vc_copylineUYVYtoRGB (:1102-1108) / YUYVtoRGB (:1116-1122).
-/// The reference computes (y_scale * (Y - 16) + c * (C - 128)) >> 14 in int32.  Every intermediate is an integer below 2^24, so the
-/// same values are formed exactly in fp32 (FFMA2 issues two lanes per slot where the integer pipe is half rate); the arithmetic
-/// shift is a round-down FMA onto the 1.5 * 2^23 magic (mantissa = floor(x / 2^14)), the clamp one VIMNMX.S16x2.RELU per two values.
-template <int Y1, int Y2, int U, int V>
-struct conv_yuv422_rgb {
-        static constexpr int IN = 32, OUT = 48;
-        static __host__ int out_len(int dst_len) { return dst_len < 6 ? 0 : dst_len / 6 * 6; }
-        static __device__ __forceinline__ float2 magic2(uint32_t w0, uint32_t w1, int byte)
-        {
-                return make_float2(__uint_as_float(__byte_perm(w0, 0x4B000000u, 0x7540u | byte)), __uint_as_float(__byte_perm(w1, 0x4B000000u, 0x7540u | byte)));
-        }
-        static __device__ __forceinline__ uint32_t floor_clamp2(float2 x)  // {clamp(x.x >> 14), clamp(x.y >> 14)} as two 16-bit lanes
-        {
-                const float2 f = __ffma2_rd(x, make_float2(0x1p-14f, 0x1p-14f), make_float2(12582912.0f, 12582912.0f));
-                return __vimin_s16x2_relu(__byte_perm(__float_as_uint(f.x), __float_as_uint(f.y), 0x5410), 0x00ff00ffu);
-        }
-        static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
-        {
-                constexpr color_coeffs c = coeffs_709(8);
-                static_assert(239L * c.y_scale + 128L * c.b_cb < (1L << 24) && 239L * c.y_scale + 128L * c.r_cr < (1L << 24), "fp32 must hold the sums exactly");
-                const float2 ys = make_float2((float) c.y_scale, (float) c.y_scale);
-#pragma unroll
-                for (int i = 0; i < 8; i += 2) {  // lanes = the same sample of words i and i + 1 (four pixels)
-                        const float2 ya = __fadd2_rn(magic2(in[i], in[i + 1], Y1), make_float2(-8388624.0f, -8388624.0f));  // Y - 16
-                        const float2 yb = __fadd2_rn(magic2(in[i], in[i + 1], Y2), make_float2(-8388624.0f, -8388624.0f));
-                        const float2 u = __fadd2_rn(magic2(in[i], in[i + 1], U), make_float2(-8388736.0f, -8388736.0f));    // Cb - 128
-                        const float2 v = __fadd2_rn(magic2(in[i], in[i + 1], V), make_float2(-8388736.0f, -8388736.0f));
-                        const float2 rc = __fmul2_rn(v, make_float2((float) c.r_cr, (float) c.r_cr));
-                        const float2 gc = __ffma2_rn(u, make_float2((float) c.g_cb, (float) c.g_cb), __fmul2_rn(v, make_float2((float) c.g_cr, (float) c.g_cr)));
-                        const float2 bc = __fmul2_rn(u, make_float2((float) c.b_cb, (float) c.b_cb));
-                        // lanes of each: {word i, word i + 1}
-                        const uint32_t r1 = floor_clamp2(__ffma2_rn(ya, ys, rc)), g1 = floor_clamp2(__ffma2_rn(ya, ys, gc)), b1 = floor_clamp2(__ffma2_rn(ya, ys, bc));
-                        const uint32_t r2 = floor_clamp2(__ffma2_rn(yb, ys, rc)), g2 = floor_clamp2(__ffma2_rn(yb, ys, gc)), b2 = floor_clamp2(__ffma2_rn(yb, ys, bc));
-                        // bytes of the 12 output bytes: word i -> r1 g1 b1 r2 g2 b2 (low lanes), word i + 1 -> the high lanes
-                        const uint32_t rg1 = __byte_perm(r1, g1, 0x6240), br = __byte_perm(b1, r2, 0x6240), gb2 = __byte_perm(g2, b2, 0x6240);  // {lo.a, lo.b, hi.a, hi.b}
-                        out[3 * (i / 2) + 0] = __byte_perm(rg1, br, 0x5410);   // r1 g1 b1 r2   (word i)
-                        out[3 * (i / 2) + 1] = __byte_perm(gb2, rg1, 0x7610);  // g2 b2 | r1' g1' (word i + 1)
-                        out[3 * (i / 2) + 2] = __byte_perm(br, gb2, 0x7632);   // b1' r2' g2' b2'
-                }
-        }
-};
-
-/// vc_copylineUYVYtoRGBA, pixfmt_conv.c:1137-1163 — the one double-precision matrix on the CPU path:
-/// products and sums in IEEE double (no contraction: the reference is built without -mfma), truncation
-/// toward zero, clamp 0..255, packed with runtime shifts + alpha mask.
-struct conv_uyvy_rgba {
-        static constexpr int IN = 16, OUT = 32;
-        static __host__ int out_len(int dst_len) { return dst_len < 8 ? 0 : dst_len / 8 * 8; }
-        // The conversions are the slow FP64 instructions on this part (I2F / F2I: 16 lanes/clk/SM against 63 for DADD/DMUL), so both go
-        // through the 2^52 magic: 2^52 + byte is exact, and x + 1.5 * 2^52 rounded toward zero leaves floor(x) in the low word - equal to
-        // the reference's truncation for x >= 0, and below zero both end at 0 after the clamp.
-        static __device__ __forceinline__ double byte_minus(uint32_t b, double bias) { return __dadd_rn(__hiloint2double(0x43300000, (int) b), bias); }
-        static __device__ __forceinline__ int trunc_int(double x) { return __double2loint(__dadd_rz(x, 6755399441055744.0)); }
-        static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &p, const row_ctx &)
-        {
-                const uint32_t amask = 0xFFFFFFFFu ^ (0xFFu << p.rshift) ^ (0xFFu << p.gshift) ^ (0xFFu << p.bshift);
-                // byte-aligned shifts (every caller in the tree): one permute places the three clamped components, selector built once per thread
-                const bool aligned = !((p.rshift | p.gshift | p.bshift) & 7);
-                uint32_t sel = 0;
-#pragma unroll
-                for (int j = 0; j < 4; ++j) {
-                        sel |= (8 * j == p.rshift ? 0u : 8 * j == p.gshift ? 2u : 8 * j == p.bshift ? 4u : 5u) << (4 * j);
-                }
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                        const uint32_t w = in[i];
-                        const double du = byte_minus(w & 0xff, -4503599627370624.0), dv = byte_minus((w >> 16) & 0xff, -4503599627370624.0);  // - (2^52 + 128)
-                        const double rv = __dmul_rn(1.793, dv), gv = __dmul_rn(0.534, dv), gu = __dmul_rn(0.213, du), bu = __dmul_rn(2.115, du);
-#pragma unroll
-                        for (int k = 0; k < 2; ++k) {
-                                const double yy = __dmul_rn(1.164, byte_minus((w >> (8 + 16 * k)) & 0xff, -4503599627370512.0));  // - (2^52 + 16)
-                                const int r = trunc_int(__dadd_rn(yy, rv)), g = trunc_int(__dadd_rn(__dadd_rn(yy, -gv), -gu)), b = trunc_int(__dadd_rn(yy, bu));
-                                // clamp 0..255 two at a time (the values fit 16 bits): VIMNMX.S16x2.RELU
-                                const uint32_t rg = __vimin_s16x2_relu(__byte_perm((uint32_t) r, (uint32_t) g, 0x5410), 0x00ff00ffu);
-                                const uint32_t bb = __vimin_s16x2_relu((uint32_t) b & 0xffffu, 0x00ff00ffu);
-                                out[2 * i + k] = aligned ? amask | __byte_perm(rg, bb, sel) : amask | (rg & 0xff) << p.rshift | (rg >> 16) << p.gshift | bb << p.bshift;
-                        }
                 }
         }
 };
