@@ -101,14 +101,20 @@ UGB_API int ugb200_jpeg_encoder_stage_times(ugb200_jpeg_encoder *enc, float us[4
 UGB_API int ugb200_jpeg_debug_coefficients(ugb200_jpeg_encoder *enc, const int16_t **dev_ptr, size_t *count);
 
 /* ---- decode (SURVEY.md section 8f rank 1): what src/video_decompress/gpujpeg.c:74-145,268-330 asks of libgpujpeg ---------------
- * Baseline sequential Huffman JPEG, 3 components, luma sampling 1x1 / 2x1 / 2x2, interleaved or one scan per component, restart
+ * Baseline sequential Huffman JPEG, 3 components (or 1, below), luma sampling 1x1 / 2x1 / 2x2, interleaved or one scan per component, restart
  * intervals (the unit of GPU parallelism), tables taken from the stream.  No colour transform inside the codec: a 4:2:2 / 4:2:0
  * YCbCr stream decodes to UYVY, a 4:4:4 RGB stream (Adobe transform 0) to RGB, a 4:4:4 YCbCr stream to VUYA; any other requested
  * output goes through UltraGrid's own line converters (ugb200_pixfmt_convert).
  * Also 4 components, all sampled 1x1, without an Adobe marker or with Adobe transform 0 (the GPUJPEG module's `alpha` stream): native
  * codec UGB_RGBA, samples as stored.  To RGBA with shifts (0, 8, 16): R G B A, alpha in byte 3, at any pitch; with other shifts that
  * result re-shifted by the RGBA -> RGBA line converter (vc_copylineRGBA: the unused byte becomes 0xFF).  To any other codec: the first three
- * planes as an RGB stream decodes.  Four-component streams with Adobe transform 1 or 2 (YCCK) or subsampled components return -4. */
+ * planes as an RGB stream decodes.  Four-component streams with Adobe transform 1 or 2 (YCCK) or subsampled components return -4.
+ * Also 1 component (grayscale: IR and machine-vision cameras, libavcodec's `gray` MJPEG), one scan with or without DRI; the sampling factors are
+ * ignored (T.81 A.2.2).  ugb200_jpeg_get_image_info reports components 1, h_samp = v_samp = 1, native codec UGB_UYVY.  ugb200_jpeg_decode_to decodes
+ * it as a YCbCr stream with Cb = Cr = 128 everywhere: UYVY `128 Y 128 Y`, I420 with 128-filled chroma planes, RGB / RGBA by the formula of
+ * stream_cs (Y601FULL gives R = G = B = Y; NATIVE: the BT.709 line converters).  VUYA output of a grayscale stream returns -4, as of every stream whose
+ * native codec is UYVY (there is no UYVY -> VUYA line converter).  ugb200_jpeg_decode and ugb200_jpeg_decode_cs refuse it with -4,
+ * as they always have. */
 typedef struct ugb200_jpeg_decoder ugb200_jpeg_decoder;
 struct ugb200_jpeg_image_info {
         int width, height, components;
@@ -163,6 +169,8 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *dec, const uint8_t *stream, 
  *   RGB and RGBA streams (Adobe transform 0, component ids 'R' 'G' 'B', four components) -> UGB200_JPEG_CS_RGB, whatever else they carry;
  *   else a SPIFF APP8: colour space 1 -> Y709, 4 -> Y601, 3 -> Y601FULL, 10 -> RGB, any other code -> -4, a segment too short for the field -> -3;
  *   else Adobe APP14 transform 1 -> Y601FULL; else JFIF APP0 -> Y601FULL; else (no marker) -> Y709, what UltraGrid assumes for unmarked streams.
+ *   A one-component stream never resolves to RGB: SPIFF colour space 8 (grayscale) -> Y601FULL, as UltraGrid's reader takes it
+ *   (src/utils/jpeg_reader.c:682-685), SPIFF 10 -> -4, everything else as above.
  *
  * ugb200_jpeg_decode_cs is ugb200_jpeg_decode, except that RGB and RGBA output of a YCbCr stream is converted from `color_space`:
  *   UGB200_JPEG_CS_NATIVE: the bytes of ugb200_jpeg_decode.
@@ -171,7 +179,7 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *dec, const uint8_t *stream, 
  *     16, 0, and >> a floor.  Chroma is replicated from its pixel pair (4:2:2) or quad (4:2:0), not interpolated.  RGBA places R, G and B at the
  *     shifts and sets every other bit (alpha 0xFF).  Y709 RGB output of a 4:2:2 or 4:2:0 stream is the RGB of ugb200_jpeg_decode byte for byte.
  *   UGB200_JPEG_CS_AUTO: as ugb200_jpeg_stream_color_space resolves it; a stream that declares RGB is not transformed, a refusal is returned.
- * RGB and four-component streams, and UYVY, I420 and VUYA output, keep the stream's samples in every mode (no YCbCr -> YCbCr matrix conversion).
+ * RGB and four-component streams, and UYVY, I420 and VUYA output, keep the stream's samples in every mode (ugb200_jpeg_decode_to converts those).
  * As in ugb200_jpeg_decode, RGB and RGBA rows of a 4:2:2 / 4:2:0 stream of odd width get whole pixel pairs only (DESIGN.md section 8).
  * Any other color_space returns -1.  On every error the output buffer is not touched.
  * Known limitation: this library's encoder writes JFIF APP0 on its UYVY and I420 streams although they hold BT.709 limited-range samples, so
@@ -179,6 +187,30 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *dec, const uint8_t *stream, 
 UGB_API int ugb200_jpeg_stream_color_space(const uint8_t *stream, size_t len);
 UGB_API int ugb200_jpeg_decode_cs(ugb200_jpeg_decoder *dec, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch,
                                   int out_codec, int rshift, int gshift, int bshift, int color_space);
+
+/* Decode to a colour space.  UltraGrid's receiver asks libgpujpeg for BT.709 limited-range UYVY / I420 whatever the stream holds
+ * (src/video_decompress/gpujpeg.c:103-138); a camera's JFIF stream holds full-range BT.601, so its samples have to be converted, not only packed.
+ *   stream_cs: as color_space of ugb200_jpeg_decode_cs (NATIVE, Y709, Y601, Y601FULL, AUTO).
+ *   out_cs:    NATIVE, Y709, Y601 or Y601FULL - the space that YCbCr output (UYVY, I420, VUYA) shall hold.  Anything else returns -1.
+ * RGB / RGBA output: exactly ugb200_jpeg_decode_cs(..., stream_cs); out_cs is ignored.
+ * YCbCr output of a YCbCr (or grayscale) stream: when stream_cs or out_cs is NATIVE, or both resolve to the same space, the bytes of
+ * ugb200_jpeg_decode.  Otherwise every decoded sample is converted at the stream's own sampling (nothing is resampled) and then packed as
+ * ugb200_jpeg_decode packs that sampling for that output codec - "convert, then pack":
+ *   Y'  = clamp(((m_yy * (Y - o_in) + m_yb * (Cb - 128) + m_yr * (Cr - 128) + 8192) >> 14) + o_out, 0, 255)   per luma sample, with the chroma
+ *                                                                                                             of its pair (4:2:2) or quad (4:2:0)
+ *   Cb' = clamp(((m_bb * (Cb - 128) + m_br * (Cr - 128) + 8192) >> 14) + 128, 0, 255)                          per chroma sample
+ *   Cr' = clamp(((m_rb * (Cb - 128) + m_rr * (Cr - 128) + 8192) >> 14) + 128, 0, 255)                          per chroma sample
+ * with o = 16 for Y709 and Y601, 0 for Y601FULL, `>>` a floor, and the seven coefficients round(2^14 * M), M = (RGB -> YCbCr of out_cs) *
+ * (YCbCr -> RGB of stream_cs) formed in double from the kr, kb and range scales of UltraGrid's color_space.c and rounded once
+ * (compute_ycc_matrix, csrc/color_space.h).  Chroma of the target does not depend on luma of the source, which makes the conversion exact at
+ * 4:2:2 and 4:2:0.  A grayscale stream takes the luma line alone (the chroma terms vanish).  The clamp is 0..255: UltraGrid's CLAMP_LIMITED_* are
+ * identities (color_space.h:93-94); libgpujpeg's own rounding is unpinned, the library being absent.  Each result lies within 1 of the unrounded
+ * matrix product (tests/test_jpeg_decode_yuv.py derives and checks the bound over every triple).
+ * YCbCr output of an RGB or four-component stream (or one that declares RGB under AUTO, which is never matrixed): out_cs NATIVE or Y709 give the
+ * bytes of ugb200_jpeg_decode (UltraGrid's line converters are BT.709); Y601 and Y601FULL return -4.
+ * Errors as ugb200_jpeg_decode_cs; on every error the output buffer is not touched. */
+UGB_API int ugb200_jpeg_decode_to(ugb200_jpeg_decoder *dec, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch,
+                                  int out_codec, int rshift, int gshift, int bshift, int stream_cs, int out_cs);
 
 #ifdef __cplusplus
 }

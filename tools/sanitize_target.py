@@ -147,9 +147,39 @@ if ONLY != "staged":
             for pitch in (ls, ls + 40):
                 for cs in ((None,) if out_c == 2 else (None, "native", "Y709", "Y601", "Y601full", "auto")):
                     out = torch.empty(pitch * h, dtype=torch.uint8, device="cuda")
-                    dec4.decode(s, out_c, shifts=(8, 16, 0) if out_c == 1 else (0, 8, 16), device=True, pitch=pitch, out=out, color_space=cs)
+                    try:
+                        dec4.decode(s, out_c, shifts=(8, 16, 0) if out_c == 1 else (0, 8, 16), device=True, pitch=pitch, out=out, color_space=cs)
+                    except RuntimeError:  # 4:4:4 YCbCr to RGBA without a colour space: no VUYA -> RGBA line converter (-4)
+                        assert ss == 0 and out_c == 1 and cs in (None, "native")
                     n += 1
     dec4.close()
+# JPEG decode to a YCbCr colour space (ugb200_jpeg_decode_to) and grayscale streams: the matrix phase of the fused kernel to UYVY for 4:2:2 / 4:2:0 at
+# odd and even sizes, its planar (I420) epilogue into tight buffers, the 4:4:4 plane kernel, and the two-warp grayscale form (odd block counts) to
+# UYVY, I420, RGB and RGBA, tight and pitched device destinations
+if ONLY != "staged":
+    dec5 = api.JpegDecoder()
+    streams = []
+    for ss, w, h in ((1, 333, 211), (2, 333, 211), (1, 64, 32), (2, 64, 32), (0, 37, 19)):
+        b = io.BytesIO()
+        Image.fromarray(natural_rgb(w, h, 6)).save(b, "JPEG", quality=90, subsampling=ss)
+        streams.append((b.getvalue(), w, h, ss == 0))
+    for w, h in ((333, 211), (72, 40), (9, 1), (1, 1)):
+        b = io.BytesIO()
+        Image.fromarray(natural_rgb(w, h, 6)[:, :, 1].copy(), "L").save(b, "JPEG", quality=90)
+        streams.append((b.getvalue(), w, h, False))
+    for s, w, h, is444 in streams:
+        for out_c in (2, 29, 12, 1) + ((4,) if is444 else ()):  # UYVY, I420, RGB, RGBA, VUYA
+            ls = vc_get_linesize(w, out_c)
+            size = w * h + 2 * ((w + 1) // 2) * ((h + 1) // 2) if out_c == 29 else None
+            for pitch in ((ls,) if out_c == 29 else (ls, ls + 40)):
+                for cs_in, cs_out in (("native", "native"), ("auto", "Y709"), ("Y709", "Y601full")):
+                    out = torch.empty(size or pitch * h, dtype=torch.uint8, device="cuda")
+                    try:
+                        dec5.decode_to(s, out_c, cs_in, cs_out, device=True, pitch=pitch, out=out)
+                    except RuntimeError:  # as above
+                        assert is444 and out_c == 1 and cs_in == "native"
+                    n += 1
+    dec5.close()
 # LDGM FEC: encode from host (packets of 4-, 8- and 16-byte words) and from a device frame at offsets 4 and 1 into a tight device buffer;
 # decode with losses peeling can repair (several levels) and with losses it cannot
 import ldgm_cases as lc

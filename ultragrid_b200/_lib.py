@@ -109,6 +109,7 @@ SIGNATURES = {
     "ugb200_jpeg_decoder_expect": (_i, [_vp, _i, _i]),
     "ugb200_jpeg_decode": (_i, [_vp, _vp, _sz, _vp, _i, _l, _i, _i, _i, _i]),
     "ugb200_jpeg_decode_cs": (_i, [_vp, _vp, _sz, _vp, _i, _l, _i, _i, _i, _i, _i]),
+    "ugb200_jpeg_decode_to": (_i, [_vp, _vp, _sz, _vp, _i, _l, _i, _i, _i, _i, _i, _i]),
     "ugb200_jpeg_stream_color_space": (_i, [_vp, _sz]),
     "ugb200_jpeg_debug_coefficients": (_i, [_vp, ctypes.POINTER(_vp), ctypes.POINTER(_sz)]),
     # include/ugb200_ldgm.h

@@ -368,10 +368,11 @@ class JpegDecoder:
         _check(_L.ugb200_jpeg_decoder_last_sync(self._h, ctypes.byref(st)), "ugb200_jpeg_decoder_last_sync")
         return {"scans": st.scans, "subsequences": st.subsequences, "rounds": st.rounds}
 
-    def decode(self, stream, out_codec, shifts=(0, 8, 16), device=False, pitch=0, out=None, sync=True, color_space=None):
+    def decode(self, stream, out_codec, shifts=(0, 8, 16), device=False, pitch=0, out=None, sync=True, color_space=None, out_cs=None):
         """bytes -> numpy array (host) or CUDA tensor (device=True) holding height rows of vc_get_linesize(width, out_codec) bytes.
         ``color_space`` None: ugb200_jpeg_decode (the stream's samples, RGB / RGBA through UltraGrid's line converters); else one of
-        JPEG_CS (``"native"``, ``"Y709"``, ``"Y601"``, ``"Y601full"``, ``"auto"``) or its value: ugb200_jpeg_decode_cs"""
+        JPEG_CS (``"native"``, ``"Y709"``, ``"Y601"``, ``"Y601full"``, ``"auto"``) or its value: ugb200_jpeg_decode_cs.  ``out_cs`` not None (``"native"``, ``"Y709"``, ``"Y601"``, ``"Y601full"`` or its value):
+        ugb200_jpeg_decode_to, UYVY / I420 / VUYA output converted from ``color_space`` (None: native) to ``out_cs``"""
         info = jpeg_image_info(stream)
         ls = pitch or vc_get_linesize(info.width, out_codec)
         nbytes = ls * info.height
@@ -383,17 +384,26 @@ class JpegDecoder:
                 out = torch.zeros(nbytes, dtype=torch.uint8, device="cuda")
             elif out.numel() * out.element_size() < nbytes:
                 raise ValueError(f"out holds {out.numel() * out.element_size()} bytes, the stream decodes to {nbytes}")
-            self._decode(buf, len(stream), _ptr(out), 1, ls, out_codec, shifts, color_space)
+            self._decode(buf, len(stream), _ptr(out), 1, ls, out_codec, shifts, color_space, out_cs)
             if sync:
                 self._stream.synchronize()
             return out
         import numpy as np
         out = np.zeros(nbytes, dtype=np.uint8)
-        self._decode(buf, len(stream), ctypes.c_void_p(out.ctypes.data), 0, ls, out_codec, shifts, color_space)
+        self._decode(buf, len(stream), ctypes.c_void_p(out.ctypes.data), 0, ls, out_codec, shifts, color_space, out_cs)
         return out
 
-    def _decode(self, buf, n, dst, is_device, pitch, out_codec, shifts, color_space):
-        if color_space is None:
+    def decode_to(self, stream, out_codec, stream_cs="auto", out_cs="Y709", **kw):
+        """ugb200_jpeg_decode_to: decode() with UYVY / I420 / VUYA output converted from ``stream_cs`` to the colour space ``out_cs``; RGB / RGBA
+        output is decode(color_space=stream_cs).  Also decodes grayscale streams."""
+        return self.decode(stream, out_codec, color_space=stream_cs, out_cs=out_cs, **kw)
+
+    def _decode(self, buf, n, dst, is_device, pitch, out_codec, shifts, color_space, out_cs=None):
+        to_cs = lambda c: 0 if c is None else JPEG_CS[c] if isinstance(c, str) else int(c)
+        if out_cs is not None:
+            _check(_L.ugb200_jpeg_decode_to(self._h, buf, n, dst, is_device, pitch, int(out_codec), *shifts, to_cs(color_space), to_cs(out_cs)),
+                   "ugb200_jpeg_decode_to")
+        elif color_space is None:
             _check(_L.ugb200_jpeg_decode(self._h, buf, n, dst, is_device, pitch, int(out_codec), *shifts), "ugb200_jpeg_decode")
         else:
             cs = JPEG_CS[color_space] if isinstance(color_space, str) else int(color_space)

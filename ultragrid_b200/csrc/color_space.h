@@ -83,4 +83,55 @@ static_assert(c0.cr_r == 8191 && c0.cr_g == -7441 && c0.cr_b == -750, "709/full 
 static_assert(c0.y_scale == 16384 && c0.r_cr == 25800 && c0.g_cb == -3069 && c0.g_cr == -7671 && c0.b_cb == 30402, "709/full inverse");
 }  // namespace pin
 
+// ---- YCbCr -> YCbCr between two colour spaces (ugb200_jpeg_decode_to) ------------------------------------------------------------
+//   Y'  = clamp(((yy * (Y - o_in) + yb * (Cb - 128) + yr * (Cr - 128) + 8192) >> 14) + o_out, 0, 255)
+//   Cb' = clamp(((bb * (Cb - 128) + br * (Cr - 128) + 8192) >> 14) + 128, 0, 255)
+//   Cr' = clamp(((rb * (Cb - 128) + rr * (Cr - 128) + 8192) >> 14) + 128, 0, 255)
+// The coefficients are round(2^14 * M), M = (RGB -> YCbCr of the target) * (YCbCr -> RGB of the source), formed in double from kr, kb and
+// the range scales above and rounded once (not the product of the rounded Q14 tables).  The target's chroma does not depend on the
+// source's luma: both are scaled B - Y and R - Y, and a grey source pixel (Cb = Cr = 128) has R = G = B.
+struct ycc_matrix {
+        int yy, yb, yr;
+        int bb, br;
+        int rb, rr;
+        int o_in, o_out;
+};
+
+constexpr ycc_matrix compute_ycc_matrix(double kr_s, double kb_s, int depth_s, double kr_t, double kb_t, int depth_t)
+{
+        using namespace detail;
+        const double ys = 1. / y_limit(depth_s), cs = 1. / c_limit(depth_s), kg_s = kg(kr_s, kb_s);
+        // R, G, B of the source as rows over (Y - o_in, Cb - 128, Cr - 128)
+        const double r[3] = { ys, 0., ee(kr_s) * cs };
+        const double g[3] = { ys, -kb_s * dd(kr_s, kb_s) / kg_s * cs, -kr_s * ee(kr_s) / kg_s * cs };
+        const double b[3] = { ys, dd(kr_s, kb_s) * cs, 0. };
+        const double l[3] = { kr_t * r[0] + kg(kr_t, kb_t) * g[0] + kb_t * b[0], kr_t * r[1] + kg(kr_t, kb_t) * g[1] + kb_t * b[1],
+                              kr_t * r[2] + kg(kr_t, kb_t) * g[2] + kb_t * b[2] };  // full-range luma of the target
+        const double yt = y_limit(depth_t), cb = c_limit(depth_t) / dd(kr_t, kb_t), cr = c_limit(depth_t) / ee(kr_t);
+        return ycc_matrix{ scaled(yt * l[0]),          scaled(yt * l[1]),          scaled(yt * l[2]),
+                           scaled(cb * (b[1] - l[1])), scaled(cb * (b[2] - l[2])), scaled(cr * (r[1] - l[1])), scaled(cr * (r[2] - l[2])),
+                           depth_s == 0 ? 0 : 16,      depth_t == 0 ? 0 : 16 };
+}
+
+/// the spaces in the order of UGB200_JPEG_CS_Y601, _Y601FULL, _Y709 (values 1, 2, 3 of include/ugb200_jpeg.h)
+constexpr ycc_matrix ycc_matrix_between(int cs_in, int cs_out)
+{
+        return compute_ycc_matrix(cs_in == 3 ? KR_709 : KR_601, cs_in == 3 ? KB_709 : KB_601, cs_in == 2 ? 0 : 8, cs_out == 3 ? KR_709 : KR_601,
+                                  cs_out == 3 ? KB_709 : KB_601, cs_out == 2 ? 0 : 8);
+}
+
+namespace pin {
+constexpr bool ycc_is(const ycc_matrix &m, int yy, int yb, int yr, int bb, int br, int rb, int rr, int o_in, int o_out)
+{
+        return m.yy == yy && m.yb == yb && m.yr == yr && m.bb == bb && m.br == br && m.rb == rb && m.rr == rr && m.o_in == o_in && m.o_out == o_out;
+}
+static_assert(ycc_is(ycc_matrix_between(1, 1), 16384, 0, 0, 16384, 0, 0, 16384, 16, 16), "Y601 -> Y601 is the identity");
+static_assert(ycc_is(ycc_matrix_between(2, 2), 16384, 0, 0, 16384, 0, 0, 16384, 0, 0), "Y601FULL -> Y601FULL is the identity");
+static_assert(ycc_is(ycc_matrix_between(3, 3), 16384, 0, 0, 16384, 0, 0, 16384, 16, 16), "Y709 -> Y709 is the identity");
+static_assert(ycc_is(ycc_matrix_between(2, 3), 14071, -1663, -2992, 14660, 1649, 1080, 14757, 0, 16), "JFIF -> BT.709: what a camera's MJPEG needs");
+static_assert(ycc_is(ycc_matrix_between(3, 2), 19077, 1895, 3656, 18462, -2063, -1351, 18342, 16, 0), "Y709 -> Y601FULL");
+static_assert(ycc_is(ycc_matrix_between(1, 3), 16384, -1893, -3406, 16689, 1877, 1230, 16799, 16, 16), "Y601 -> Y709");
+static_assert(ycc_is(ycc_matrix_between(2, 1), 14071, 0, 0, 14392, 0, 0, 14392, 0, 16), "Y601FULL -> Y601: a range change only");
+}  // namespace pin
+
 }  // namespace ugb

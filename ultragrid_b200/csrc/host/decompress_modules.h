@@ -8,6 +8,7 @@
 // Everything CUDA happens behind the C ABI of libugb200.so (include/*.h).
 #pragma once
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 
 #include "../../../include/cuda_dxt.h"
@@ -26,6 +27,38 @@ static int no_corrupted_frames(void *, int property, void *val, size_t *len)  //
         }
         return 0;
 }
+/// The colour space the JPEG modules take a stream's YCbCr to be, read when a module instance is created: UGB200_JPEG_DECODE_CS=auto|y709|y601|y601full
+/// makes gpujpeg and gpujpeg_to_dxt ask for BT.709 output converted from that space (what gpujpeg.c:81,103-138 asks of libgpujpeg: GPUJPEG_YCBCR_BT709
+/// for UYVY / I420, RGB converted from the stream's space).  Unset (NATIVE): the stream's samples as they are, the bytes of ugb200_jpeg_decode - this
+/// library's encoder labels its BT.709 streams with JFIF APP0, which `auto` would read as full-range BT.601.
+static int jpeg_decode_cs_from_env()
+{
+        const char *e = getenv("UGB200_JPEG_DECODE_CS");
+        if (e == nullptr || e[0] == 0) {
+                return UGB200_JPEG_CS_NATIVE;
+        }
+        if (strcmp(e, "auto") == 0) {
+                return UGB200_JPEG_CS_AUTO;
+        }
+        if (strcmp(e, "y709") == 0) {
+                return UGB200_JPEG_CS_Y709;
+        }
+        if (strcmp(e, "y601") == 0) {
+                return UGB200_JPEG_CS_Y601;
+        }
+        if (strcmp(e, "y601full") == 0) {
+                return UGB200_JPEG_CS_Y601FULL;
+        }
+        fprintf(stderr, "[GPUJPEG dec.] UGB200_JPEG_DECODE_CS=%s is not one of auto, y709, y601, y601full: ignored\n", e);
+        return UGB200_JPEG_CS_NATIVE;
+}
+/// ugb200_jpeg_decode_to with the module's colour space: NATIVE gives the bytes of ugb200_jpeg_decode (and decodes grayscale streams, which that call refuses)
+static int jpeg_module_decode(ugb200_jpeg_decoder *dec, int stream_cs, const unsigned char *buffer, size_t len, void *dst, int dst_is_device, long pitch, int out_codec,
+                              int rshift, int gshift, int bshift)
+{
+        return ugb200_jpeg_decode_to(dec, buffer, len, dst, dst_is_device, pitch, out_codec, rshift, gshift, bshift, stream_cs,
+                                     stream_cs == UGB200_JPEG_CS_NATIVE ? UGB200_JPEG_CS_NATIVE : UGB200_JPEG_CS_Y709);
+}
 
 // ---- gpujpeg ---------------------------------------------------------------------------------------------------------------------
 #if UGB_DECOMPRESS_MODULES & 1
@@ -35,6 +68,7 @@ struct state_decompress_gpujpeg {  // gpujpeg.c:63-70
         struct video_desc desc{};
         int rshift = 0, gshift = 0, bshift = 0, pitch = 0;
         codec_t out_codec = VIDEO_CODEC_NONE;
+        int stream_cs = jpeg_decode_cs_from_env();
 };
 }  // namespace
 
@@ -81,7 +115,7 @@ static decompress_status gpujpeg_decompress(void *state, unsigned char *dst, uns
         }
         cuda_wrapper_set_device((int) cuda_devices[0]);
         // the device path writes any pitch and any RGBA shifts directly (the reference needs a second CPU pass for those, gpujpeg.c:295-318)
-        const int rc = ugb200_jpeg_decode(s->decoder, buffer, src_len, dst, 0, s->pitch, s->out_codec, s->rshift, s->gshift, s->bshift);
+        const int rc = jpeg_module_decode(s->decoder, s->stream_cs, buffer, src_len, dst, 0, s->pitch, s->out_codec, s->rshift, s->gshift, s->bshift);
         return rc == 0 ? DECODER_GOT_FRAME : DECODER_NO_FRAME;
 }
 static void gpujpeg_decompress_done(void *state)
@@ -112,6 +146,7 @@ struct state_gpujpeg_to_dxt {
         ugb200_jpeg_decoder *decoder = nullptr;
         void *rgb = nullptr, *dxt = nullptr;  // device
         size_t rgb_cap = 0, dxt_cap = 0;
+        int stream_cs = jpeg_decode_cs_from_env();
         struct video_desc desc{};
         codec_t out_codec = VIDEO_CODEC_NONE;
 };
@@ -159,7 +194,7 @@ static decompress_status gpujpeg_to_dxt_decompress(void *state, unsigned char *d
 {
         auto *s = (state_gpujpeg_to_dxt *) state;
         cuda_wrapper_set_device((int) cuda_devices[0]);
-        if (ugb200_jpeg_decode(s->decoder, buffer, src_len, s->rgb, 1, 0, RGB, 0, 8, 16) != 0) {
+        if (jpeg_module_decode(s->decoder, s->stream_cs, buffer, src_len, s->rgb, 1, 0, RGB, 0, 8, 16) != 0) {
                 return DECODER_NO_FRAME;
         }
         const int w = (int) s->desc.width, h = (int) s->desc.height;

@@ -590,6 +590,8 @@ struct epi_uyvy {
         static constexpr int PX = 8, OUT = 16, BPP = 2;
         static __device__ __forceinline__ void run(const uint32_t *w, uint32_t *o, const conv_params &) { o[0] = w[0], o[1] = w[1], o[2] = w[2], o[3] = w[3]; }
 };
+/// I420 output: the kernel writes the three planes from its tile (its planar epilogue); the constants only size the unused packed path
+struct epi_i420 : epi_uyvy {};
 /// RGB / RGBA output: a line converter functor (yuv_rgb_conv.cuh) applied to the UYVY words of 16 pixels, as ugb200_pixfmt_convert would apply it
 /// to the UYVY frame
 template <class C>
@@ -624,11 +626,19 @@ __device__ __forceinline__ void uyvy_words(uint2 Y, uint32_t C, uint32_t R, uint
 /// converted to RGB / RGBA, 16 pixels per thread, staged per warp in shared memory so that each warp stores its row's run as consecutive 16-byte
 /// pieces.  Same IDCT arithmetic as jpeg_idct_kernel.  A row holds ((w + 1) / 2) * 4 bytes of UYVY (the last pair of an odd width takes the padded
 /// plane's luma) but only whole pixel pairs of RGB / RGBA (the line converters' out_len), and rows but the last stop at the pitch, as there.
-template <int V, class E>
-__global__ void __launch_bounds__(32 * (2 * V + 2)) jpeg_idct_packed_kernel(const int16_t *__restrict__ coef, const dec_tables *__restrict__ tables, dec_geom g,
-                                                                            uint8_t *__restrict__ out, long pitch, bool vec_ok, conv_params p)
+/// MX: the samples are taken from one YCbCr colour space to another (ycc_matrix, color_space.h) in the shared tile before they are packed - luma
+/// first, with the source chroma of its pair / quad, then each chroma sample once - so the epilogue and its stores are those of the plain kernel.
+/// E = epi_i420: `out` is a tight I420 frame (Y plane of w x h, then Cb and Cr of (w + 1) / 2 x (h + 1) / 2).  Luma rows leave the tile as 8-byte pieces,
+/// consecutive threads consecutive in memory.  A 4:2:0 stream's chroma tiles ARE the I420 chroma (uyvy_to_i420(yuv420p_to_uyvy(x)) = x); a 4:2:2 stream's
+/// chroma rows are averaged in pairs, (a + b + 1) / 2, as uyvy_to_i420 does (to_planar.c:364-367) - an MCU row is 8 pixel rows, so a pair never straddles
+/// CTAs - and the last row of an odd height is taken as it is.  With MX the averaged samples are the converted ones ("convert, then pack").
+/// GRAY: a one-component stream (V = 1): the CTA is 32 pairs of luma blocks of a block row, two warps, and the epilogues are fed Cb = Cr = 128.
+template <int V, class E, bool MX = false, bool GRAY = false>
+__global__ void __launch_bounds__(32 * (GRAY ? 2 : 2 * V + 2)) jpeg_idct_packed_kernel(const int16_t *__restrict__ coef, const dec_tables *__restrict__ tables, dec_geom g,
+                                                                                       uint8_t *__restrict__ out, long pitch, bool vec_ok, conv_params p, ycc_matrix ym)
 {
-        constexpr int NB = 2 * V + 2, NT = 32 * NB, ROWS = 8 * V, PPR = 32 * 16 / E::PX;  // blocks per MCU, threads, pixel rows, pieces per row
+        static_assert(!GRAY || V == 1, "a one-component scan is not interleaved: its MCU is one block");
+        constexpr int NB = GRAY ? 2 : 2 * V + 2, NT = 32 * NB, ROWS = 8 * V, PPR = 32 * 16 / E::PX;  // blocks per MCU, threads, pixel rows, pieces per row
         constexpr bool STAGED = E::PX == 16;
         __shared__ float s_m[4][64];
         __shared__ uint2 s_tile[NB][8][32];
@@ -638,9 +648,9 @@ __global__ void __launch_bounds__(32 * (2 * V + 2)) jpeg_idct_packed_kernel(cons
                 s_m[i >> 6][i & 63] = tables->m[i >> 6][i & 63];
         }
         __syncthreads();
-        const int mcux = g.c[1].bw, my = blockIdx.y, mx0 = blockIdx.x * 32;
+        const int mcux = GRAY ? (g.c[0].bw + 1) / 2 : g.c[1].bw, my = blockIdx.y, mx0 = blockIdx.x * 32;
         const int k = tid >> 5, lane = tid & 31, mx = mx0 + lane;
-        if (mx < mcux) {
+        if (mx < mcux && (!GRAY || 2 * mx + k < g.c[0].bw)) {  // GRAY: an odd block count leaves the last pair's second block out (it lies past the width)
                 const int ci = k < 2 * V ? 0 : k - 2 * V + 1;
                 const dec_comp &c = g.c[ci];
                 const int X = ci == 0 ? 2 * mx + (k & 1) : mx, Y = ci == 0 ? V * my + (k >> 1) : my;
@@ -676,6 +686,93 @@ __global__ void __launch_bounds__(32 * (2 * V + 2)) jpeg_idct_packed_kernel(cons
                 }
         }
         __syncthreads();
+        if constexpr (MX) {
+                const int ybias = 8192 - ym.yy * ym.o_in;
+                auto conv4 = [&](uint32_t y, int t0, int t1) {  // four luma samples, two pairs
+                        uint32_t r = 0;
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                                const int v = ((ym.yy * (int) ((y >> (8 * i)) & 0xffu) + (i < 2 ? t0 : t1)) >> 14) + ym.o_out;
+                                r |= (uint32_t) min(max(v, 0), 255) << (8 * i);
+                        }
+                        return r;
+                };
+                for (int i = tid; i < 2 * V * 256; i += NT) {  // luma: 8 samples of a block row with the 4 chroma pairs above them
+                        const int mcu = i & 31, r = (i >> 5) & 7, kb = i >> 8;
+                        int t[4] = { ybias, ybias, ybias, ybias };
+                        if constexpr (!GRAY) {
+                                const int crow = V == 2 ? 4 * (kb >> 1) + (r >> 1) : r;
+                                const uint2 CB = s_tile[2 * V][crow][mcu], CR = s_tile[2 * V + 1][crow][mcu];
+                                const uint32_t cb = kb & 1 ? CB.y : CB.x, cr = kb & 1 ? CR.y : CR.x;
+#pragma unroll
+                                for (int j = 0; j < 4; ++j) {
+                                        t[j] += ym.yb * ((int) ((cb >> (8 * j)) & 0xffu) - 128) + ym.yr * ((int) ((cr >> (8 * j)) & 0xffu) - 128);
+                                }
+                        }
+                        const uint2 y = s_tile[kb][r][mcu];
+                        s_tile[kb][r][mcu] = make_uint2(conv4(y.x, t[0], t[1]), conv4(y.y, t[2], t[3]));
+                }
+                if constexpr (!GRAY) {
+                        __syncthreads();  // every luma sample has read its source chroma
+                        for (int i = tid; i < 512; i += NT) {  // chroma: four samples of Cb and of Cr at the same place
+                                const int mcu = i & 31, r = (i >> 5) & 7, half = i >> 8;
+                                uint32_t *pb = (uint32_t *) &s_tile[2 * V][r][mcu] + half, *pr = (uint32_t *) &s_tile[2 * V + 1][r][mcu] + half;
+                                const uint32_t cb = *pb, cr = *pr;
+                                uint32_t ob = 0, orr = 0;
+#pragma unroll
+                                for (int j = 0; j < 4; ++j) {
+                                        const int b = (int) ((cb >> (8 * j)) & 0xffu) - 128, r2 = (int) ((cr >> (8 * j)) & 0xffu) - 128;
+                                        ob |= (uint32_t) min(max(((ym.bb * b + ym.br * r2 + 8192) >> 14) + 128, 0), 255) << (8 * j);
+                                        orr |= (uint32_t) min(max(((ym.rb * b + ym.rr * r2 + 8192) >> 14) + 128, 0), 255) << (8 * j);
+                                }
+                                *pb = ob, *pr = orr;
+                        }
+                }
+                __syncthreads();
+        }
+        if constexpr (std::is_same<E, epi_i420>::value) {
+                const int cw = (g.w + 1) / 2, chh = (g.h + 1) / 2;
+                auto store8 = [&](uint8_t *row, int x, int width, uint2 v) {  // 8 samples at row[x], cut at the plane's width
+                        if (x >= width) {
+                                return;
+                        }
+                        if (vec_ok && x + 8 <= width) {
+                                *(uint2 *) (row + x) = v;
+                        } else {
+                                for (int b = 0; b < 8 && x + b < width; ++b) {
+                                        row[x + b] = (uint8_t) ((b < 4 ? v.x : v.y) >> (8 * (b & 3)));
+                                }
+                        }
+                };
+                for (int i = tid; i < ROWS * 64; i += NT) {  // luma: 64 pieces of 8 pixels per row
+                        const int row = i >> 6, piece = i & 63, mcu = piece >> 1, y = my * ROWS + row;
+                        if (y < g.h && mx0 + mcu < mcux) {
+                                store8(out + (long) y * g.w, (mx0 + mcu) * 16 + (piece & 1) * 8, g.w, s_tile[(V == 2 ? 2 * (row >> 3) : 0) + (piece & 1)][row & 7][mcu]);
+                        }
+                }
+                constexpr int CROWS = V == 2 ? 8 : 4;  // chroma rows of the MCU row
+                uint8_t *const cplane = out + (long) g.w * g.h;
+                for (int i = tid; i < 2 * CROWS * 32; i += NT) {
+                        const int mcu = i & 31, r = (i >> 5) % CROWS, comp = i / (32 * CROWS), cy = my * CROWS + r;
+                        if (cy >= chh || mx0 + mcu >= mcux) {
+                                continue;
+                        }
+                        uint2 v = make_uint2(0x80808080u, 0x80808080u);
+                        if constexpr (!GRAY) {
+                                if (V == 2) {
+                                        v = s_tile[4 + comp][r][mcu];
+                                } else {
+                                        v = s_tile[2 + comp][2 * r][mcu];
+                                        if (my * 8 + 2 * r + 1 < g.h) {
+                                                const uint2 b = s_tile[2 + comp][2 * r + 1][mcu];
+                                                v = make_uint2(__vavgu4(v.x, b.x), __vavgu4(v.y, b.y));
+                                        }
+                                }
+                        }
+                        store8(cplane + (long) comp * cw * chh + (long) cy * cw, (mx0 + mcu) * 8, cw, v);
+                }
+                return;
+        }
         const int row_full = E::BPP == 2 ? ((g.w + 1) / 2) * 4 : (g.w / 2) * 2 * E::BPP;
         for (int cidx = tid; cidx < ROWS * PPR; cidx += NT) {
                 const int row = cidx / PPR, piece = cidx % PPR, mcu = piece / (16 / E::PX), half = piece % (16 / E::PX);
@@ -685,7 +782,12 @@ __global__ void __launch_bounds__(32 * (2 * V + 2)) jpeg_idct_packed_kernel(cons
                 }
                 const int lim = E::BPP == 2 || y == g.h - 1 || row_full <= pitch ? row_full : (int) pitch;
                 const int cb = 2 * V, crow = V == 2 ? row >> 1 : row, yb = V == 2 ? 2 * (row >> 3) : 0, yrow = row & 7;
-                const uint2 CB = s_tile[cb][crow][mcu], CR = s_tile[cb + 1][crow][mcu];
+                uint2 CB, CR;
+                if constexpr (GRAY) {
+                        CB = CR = make_uint2(0x80808080u, 0x80808080u);
+                } else {
+                        CB = s_tile[cb][crow][mcu], CR = s_tile[cb + 1][crow][mcu];
+                }
                 uint32_t w[E::PX / 2], o[E::OUT / 4];
                 if (E::PX == 8) {
                         uyvy_words(s_tile[yb + half][yrow][mcu], half ? CB.y : CB.x, half ? CR.y : CR.x, w);
@@ -760,6 +862,27 @@ __global__ void __launch_bounds__(256) jpeg_planes_cs_kernel(const uint8_t *__re
         } else {
                 d[3 * x] = (uint8_t) r, d[3 * x + 1] = (uint8_t) gg, d[3 * x + 2] = (uint8_t) b;
         }
+}
+
+/// 4:4:4 YCbCr streams from one YCbCr colour space to another (ycc_matrix): the three component planes of jpeg_idct_kernel in place, four samples
+/// per thread, before the packers read them (same integers as the MX phase of jpeg_idct_packed_kernel)
+__global__ void __launch_bounds__(256) jpeg_planes_ycc_kernel(uint8_t *__restrict__ planes, dec_geom g, ycc_matrix ym)
+{
+        const long i = (long) blockIdx.x * blockDim.x + threadIdx.x;
+        if (i >= (long) g.c[0].bw * g.c[0].bh * 16) {  // 1x1 sampling: the three padded planes have the same size, a multiple of 64
+                return;
+        }
+        uint32_t *py = (uint32_t *) (planes + g.c[0].plane_off) + i, *pb = (uint32_t *) (planes + g.c[1].plane_off) + i, *pr = (uint32_t *) (planes + g.c[2].plane_off) + i;
+        const uint32_t y = *py, cb = *pb, cr = *pr;
+        uint32_t oy = 0, ob = 0, orr = 0;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+                const int Y = (int) ((y >> (8 * j)) & 0xffu) - ym.o_in, b = (int) ((cb >> (8 * j)) & 0xffu) - 128, r = (int) ((cr >> (8 * j)) & 0xffu) - 128;
+                oy |= (uint32_t) min(max(((ym.yy * Y + ym.yb * b + ym.yr * r + 8192) >> 14) + ym.o_out, 0), 255) << (8 * j);
+                ob |= (uint32_t) min(max(((ym.bb * b + ym.br * r + 8192) >> 14) + 128, 0), 255) << (8 * j);
+                orr |= (uint32_t) min(max(((ym.rb * b + ym.rr * r + 8192) >> 14) + 128, 0), 255) << (8 * j);
+        }
+        *py = oy, *pb = ob, *pr = orr;
 }
 
 // ---- marker scan on the device (streams with one interleaved scan: what UltraGrid sends for UYVY; or one scan per component: RGB) ---------------
@@ -1085,6 +1208,11 @@ bool hgrow(T *&ptr, size_t &cap, size_t need)
 
 int be16(const uint8_t *p) { return p[0] << 8 | p[1]; }
 
+template <class T>
+struct type_tag {  // carries an epilogue type into a generic lambda
+        using type = T;
+};
+
 constexpr long kMaxPixels = 16384L * 16384L;  // four 8K frames side by side; larger SOF dimensions are refused before anything is allocated
 
 struct huff_defs {  // the current DHT definition of each table id, built into a slot of dec_tables when a scan first uses it
@@ -1281,7 +1409,7 @@ int parse_stream(const uint8_t *s, size_t len, parsed &P, dec_tables *T, bool fu
                                 return -4;
                         }
                         g.h = be16(d + 1), g.w = be16(d + 3), g.ncomp = d[5];
-                        if ((g.ncomp != 3 && g.ncomp != 4) || g.w == 0 || g.h == 0) {
+                        if ((g.ncomp != 1 && g.ncomp != 3 && g.ncomp != 4) || g.w == 0 || g.h == 0) {
                                 return -4;
                         }
                         if ((long) g.w * g.h > kMaxPixels) {  // header fields are untrusted: they size every host and device allocation below
@@ -1291,6 +1419,9 @@ int parse_stream(const uint8_t *s, size_t len, parsed &P, dec_tables *T, bool fu
                         for (int i = 0; i < g.ncomp; ++i) {
                                 P.comp_id[i] = d[6 + 3 * i];
                                 g.c[i].h = d[7 + 3 * i] >> 4, g.c[i].v = d[7 + 3 * i] & 15, g.c[i].tq = d[8 + 3 * i];
+                                if (g.ncomp == 1) {  // T.81 A.2.2: a single-component scan is never interleaved, its sampling factors have no effect
+                                        g.c[i].h = g.c[i].v = 1;
+                                }
                                 g.hmax = g.c[i].h > g.hmax ? g.c[i].h : g.hmax, g.vmax = g.c[i].v > g.vmax ? g.c[i].v : g.vmax;
                         }
                         int blk = 0;
@@ -1442,8 +1573,8 @@ int native_codec(const parsed &P)
         if (g.ncomp == 4) {
                 return UGB_RGBA;  // R G B A as stored (the parser refuses subsampled and YCCK four-component streams)
         }
-        if (g.c[0].h == 2) {
-                return UGB_UYVY;  // 4:2:2 and 4:2:0 land in UYVY
+        if (g.c[0].h == 2 || g.ncomp == 1) {
+                return UGB_UYVY;  // 4:2:2 and 4:2:0 land in UYVY; so does grayscale, with Cb = Cr = 128
         }
         const bool rgb = P.adobe == 0 || (P.comp_id[0] == 'R' && P.comp_id[1] == 'G' && P.comp_id[2] == 'B');
         return rgb ? UGB_RGB : UGB_VUYA;
@@ -1457,6 +1588,9 @@ int declared_color_space(const parsed &P)
                 return UGB200_JPEG_CS_RGB;
         }
         if (P.spiff != -1) {  // SPIFF colour space codes (ITU-T T.84 Annex F)
+                if (P.g.ncomp == 1 && (P.spiff == 8 || P.spiff == 10)) {  // grayscale is full-range luma; a one-component stream is never RGB
+                        return P.spiff == 8 ? UGB200_JPEG_CS_Y601FULL : -4;
+                }
                 switch (P.spiff) {
                 case -2: return -3;
                 case 1: return UGB200_JPEG_CS_Y709;
@@ -1635,9 +1769,10 @@ UGB_API int ugb200_jpeg_decoder_expect(ugb200_jpeg_decoder *d, int width, int he
         return 0;
 }
 
-/// ugb200_jpeg_decode and ugb200_jpeg_decode_cs: color_space is one of NATIVE, Y601, Y601FULL, Y709, AUTO
+/// ugb200_jpeg_decode, ugb200_jpeg_decode_cs and ugb200_jpeg_decode_to: color_space is one of NATIVE, Y601, Y601FULL, Y709, AUTO; out_cs (the space of
+/// UYVY, I420 and VUYA output) one of NATIVE, Y601, Y601FULL, Y709; gray_ok: one-component streams are decoded (ugb200_jpeg_decode_to), else -4 as ever
 static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec, int rshift, int gshift,
-                  int bshift, int color_space)
+                  int bshift, int color_space, int out_cs, bool gray_ok = false)
 {
         const long dst_pitch_arg = dst_pitch;
         if (!d || !stream || !dst || len > 0xFFFFFFF0u) {
@@ -1769,6 +1904,9 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
                 P.g.ntables = P.hd.taken[k] ? k + 1 : P.g.ntables;
         }
         const dec_geom &g = P.g;
+        if (g.ncomp == 1 && !gray_ok) {
+                return -4;
+        }
         const size_t nseg = multi ? (size_t) (g.s[2].seg0 + g.s[2].nseg) : device_scan ? (size_t) g.s[0].nseg : P.seg_begin.size();
         d->last_nseg = nseg;
         const long plane_bytes = (long) g.nblocks * 64;
@@ -1788,6 +1926,15 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
         }
         const int conv_cs = (native == UGB_UYVY || native == UGB_VUYA) && (out_codec == UGB_RGB || out_codec == UGB_RGBA) && cs != UGB200_JPEG_CS_RGB ? cs
                                                                                                                                                : UGB200_JPEG_CS_NATIVE;
+        // UYVY, I420 and VUYA output in a colour space (ugb200_jpeg_decode_to): a YCbCr stream's samples go through the matrix between the two spaces
+        // before they are packed.  RGB and four-component streams reach YCbCr through UltraGrid's BT.709 line converters only.
+        const bool ycc_out = out_codec == UGB_UYVY || out_codec == UGB_I420 || out_codec == UGB_VUYA;
+        const bool ycc_stream = (native == UGB_UYVY || native == UGB_VUYA) && cs != UGB200_JPEG_CS_RGB;
+        if (ycc_out && !ycc_stream && (out_cs == UGB200_JPEG_CS_Y601 || out_cs == UGB200_JPEG_CS_Y601FULL)) {
+                return -4;
+        }
+        const bool matrix = ycc_out && ycc_stream && cs != UGB200_JPEG_CS_NATIVE && out_cs != UGB200_JPEG_CS_NATIVE && cs != out_cs;
+        const ycc_matrix ym = matrix ? ycc_matrix_between(cs, out_cs) : ycc_matrix{};
         if (dst_pitch == 0) {
                 dst_pitch = opitch;
         }
@@ -1831,7 +1978,7 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
                         lap("verdict");
                         if (*d->h_flag != 0) {
                                 d->host_once = true;
-                                return decode(d, stream, len, dst, dst_is_device, dst_pitch_arg, out_codec, rshift, gshift, bshift, color_space);
+                                return decode(d, stream, len, dst, dst_is_device, dst_pitch_arg, out_codec, rshift, gshift, bshift, color_space, out_cs, gray_ok);
                         }
                 } else {
                         jpeg_marker_segments_kernel<<<(unsigned) ((nseg + 255) / 256), 256, 0, s>>>(d->d_marks, meta, (uint32_t) scan_data, (uint32_t) len, (int) nseg, d->d_seg,
@@ -1862,7 +2009,9 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
                                 full = full && S.mcux == c.bw && S.nmcu == c.bw * c.bh;
                         }
                 }
-                full = full && seen[0] == 1 && seen[1] == 1 && seen[2] == 1 && (g.ncomp == 3 || seen[3] == 1);
+                for (int i = 0; i < g.ncomp; ++i) {
+                        full = full && seen[i] == 1;
+                }
         }
         const unsigned hgrid = (unsigned) ((nseg + kHuffThreads - 1) / kHuffThreads);
         const size_t hsmem = kTablesSmem + (size_t) kHuffThreads * 128;
@@ -1939,41 +2088,52 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
         uint8_t *const conv = dst_is_device ? (uint8_t *) dst : d->staging;
         const long cpitch = dst_is_device ? dst_pitch : opitch;
         const conv_params cp = { rshift, gshift, bshift, 0 };
+        // I420 of a 4:2:2, 4:2:0 or grayscale stream: the fused kernel writes the three tight planes (GPUJPEG_420_U8_P0P1P2, gpujpeg.c:113-116) itself
+        const bool planar = fused && out_codec == UGB_I420;
+        const size_t i420_bytes = (size_t) g.w * g.h + 2 * (size_t) ((g.w + 1) / 2) * ((g.h + 1) / 2);
+        if (planar && !dst_is_device && !dgrow(d->staging, d->staging_cap, i420_bytes + 64)) {
+                return -2;
+        }
         if (fused) {  // 4:2:2 and 4:2:0: IDCT, chroma replication and packing (or conversion) in one kernel, no component planes
                 const bool uyvy_out = !to_out;
-                uint8_t *o = uyvy_out ? nat : conv;
-                const long op = uyvy_out ? (direct ? dst_pitch : npitch) : cpitch;
-                const dim3 grid((unsigned) ((g.c[1].bw + 31) / 32), (unsigned) g.c[1].bh);
+                uint8_t *o = planar ? (dst_is_device ? (uint8_t *) dst : d->staging) : uyvy_out ? nat : conv;
+                const long op = planar ? g.w : uyvy_out ? (direct ? dst_pitch : npitch) : cpitch;
+                const bool gray = g.ncomp == 1;
+                const dim3 grid((unsigned) (((gray ? (g.c[0].bw + 1) / 2 : g.c[1].bw) + 31) / 32), (unsigned) (gray ? g.c[0].bh : g.c[1].bh));
                 const bool vec = !(15 & (size_t) o) && !(op & 15);
-                const int kind = uyvy_out ? 0 : out_codec == UGB_RGB ? (conv_cs == UGB200_JPEG_CS_NATIVE ? UGB200_JPEG_CS_Y709 : conv_cs) : 4 + conv_cs;
-                auto launch = [&](auto v) {
+                const int kind = planar ? 8 : uyvy_out ? 0 : out_codec == UGB_RGB ? (conv_cs == UGB200_JPEG_CS_NATIVE ? UGB200_JPEG_CS_Y709 : conv_cs) : 4 + conv_cs;
+                auto launch = [&](auto v, auto gr) {
                         constexpr int V = decltype(v)::value;
+                        constexpr bool G = decltype(gr)::value;
+                        constexpr int NT = 32 * (G ? 2 : 2 * V + 2);
+                        auto run = [&](auto e, auto m) {
+                                jpeg_idct_packed_kernel<V, typename decltype(e)::type, decltype(m)::value, G><<<grid, NT, 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp, ym);
+                        };
+                        const std::false_type plain;
                         switch (kind) {
-                        case 0: jpeg_idct_packed_kernel<V, epi_uyvy><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp); break;
-                        case UGB200_JPEG_CS_Y709: jpeg_idct_packed_kernel<V, epi_rgb><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp); break;
-                        case UGB200_JPEG_CS_Y601: jpeg_idct_packed_kernel<V, epi_cs_rgb<ycbcr_601>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp); break;
-                        case UGB200_JPEG_CS_Y601FULL:
-                                jpeg_idct_packed_kernel<V, epi_cs_rgb<ycbcr_601_full>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp);
-                                break;
-                        case 4 + UGB200_JPEG_CS_NATIVE: jpeg_idct_packed_kernel<V, epi_rgba><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp); break;
-                        case 4 + UGB200_JPEG_CS_Y709:
-                                jpeg_idct_packed_kernel<V, epi_cs_rgba<ycbcr_709>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp);
-                                break;
-                        case 4 + UGB200_JPEG_CS_Y601:
-                                jpeg_idct_packed_kernel<V, epi_cs_rgba<ycbcr_601>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp);
-                                break;
-                        default:
-                                jpeg_idct_packed_kernel<V, epi_cs_rgba<ycbcr_601_full>><<<grid, 32 * (2 * V + 2), 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp);
-                                break;
+                        case 0: matrix ? run(type_tag<epi_uyvy>(), std::true_type()) : run(type_tag<epi_uyvy>(), plain); break;
+                        case UGB200_JPEG_CS_Y709: run(type_tag<epi_rgb>(), plain); break;
+                        case UGB200_JPEG_CS_Y601: run(type_tag<epi_cs_rgb<ycbcr_601>>(), plain); break;
+                        case UGB200_JPEG_CS_Y601FULL: run(type_tag<epi_cs_rgb<ycbcr_601_full>>(), plain); break;
+                        case 4 + UGB200_JPEG_CS_NATIVE: run(type_tag<epi_rgba>(), plain); break;
+                        case 4 + UGB200_JPEG_CS_Y709: run(type_tag<epi_cs_rgba<ycbcr_709>>(), plain); break;
+                        case 4 + UGB200_JPEG_CS_Y601: run(type_tag<epi_cs_rgba<ycbcr_601>>(), plain); break;
+                        case 8: matrix ? run(type_tag<epi_i420>(), std::true_type()) : run(type_tag<epi_i420>(), plain); break;
+                        default: run(type_tag<epi_cs_rgba<ycbcr_601_full>>(), plain); break;
                         }
                 };
-                if (g.c[0].v == 2) {
-                        launch(std::integral_constant<int, 2>());
+                if (gray) {
+                        launch(std::integral_constant<int, 1>(), std::true_type());
+                } else if (g.c[0].v == 2) {
+                        launch(std::integral_constant<int, 2>(), std::false_type());
                 } else {
-                        launch(std::integral_constant<int, 1>());
+                        launch(std::integral_constant<int, 1>(), std::false_type());
                 }
         } else {
                 jpeg_idct_kernel<<<(g.nblocks + 127) / 128, 128, 0, s>>>(d->coef, d->d_tables, g, d->planes);
+                if (matrix) {
+                        jpeg_planes_ycc_kernel<<<(unsigned) (((long) g.c[0].bw * g.c[0].bh * 16 + 255) / 256), 256, 0, s>>>(d->planes, g, ym);
+                }
                 if (to_out) {  // 4:4:4 YCbCr in a colour space: per pixel over the planes
                         const dim3 grid((unsigned) ((g.w + 255) / 256), (unsigned) g.h);
                         const bool rgba = out_codec == UGB_RGBA;
@@ -1994,6 +2154,12 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
         }
         lap("kernels queued");
         lap("+huffman + idct");
+        if (planar) {
+                if (dst_is_device) {
+                        return 0;
+                }
+                return cudaMemcpyAsync(dst, d->staging, i420_bytes, cudaMemcpyDeviceToHost, s) == cudaSuccess && cudaStreamSynchronize(s) == cudaSuccess ? 0 : -2;
+        }
         if (to_out) {
                 if (dst_is_device) {
                         return 0;
@@ -2097,7 +2263,7 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
 UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec,
                                int rshift, int gshift, int bshift)
 {
-        return decode(d, stream, len, dst, dst_is_device, dst_pitch, out_codec, rshift, gshift, bshift, UGB200_JPEG_CS_NATIVE);
+        return decode(d, stream, len, dst, dst_is_device, dst_pitch, out_codec, rshift, gshift, bshift, UGB200_JPEG_CS_NATIVE, UGB200_JPEG_CS_NATIVE);
 }
 
 UGB_API int ugb200_jpeg_decode_cs(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec,
@@ -2107,7 +2273,20 @@ UGB_API int ugb200_jpeg_decode_cs(ugb200_jpeg_decoder *d, const uint8_t *stream,
             color_space != UGB200_JPEG_CS_Y709 && color_space != UGB200_JPEG_CS_AUTO) {
                 return -1;
         }
-        return decode(d, stream, len, dst, dst_is_device, dst_pitch, out_codec, rshift, gshift, bshift, color_space);
+        return decode(d, stream, len, dst, dst_is_device, dst_pitch, out_codec, rshift, gshift, bshift, color_space, UGB200_JPEG_CS_NATIVE);
+}
+
+UGB_API int ugb200_jpeg_decode_to(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec,
+                                  int rshift, int gshift, int bshift, int stream_cs, int out_cs)
+{
+        if (stream_cs != UGB200_JPEG_CS_NATIVE && stream_cs != UGB200_JPEG_CS_Y601 && stream_cs != UGB200_JPEG_CS_Y601FULL && stream_cs != UGB200_JPEG_CS_Y709 &&
+            stream_cs != UGB200_JPEG_CS_AUTO) {
+                return -1;
+        }
+        if (out_cs != UGB200_JPEG_CS_NATIVE && out_cs != UGB200_JPEG_CS_Y601 && out_cs != UGB200_JPEG_CS_Y601FULL && out_cs != UGB200_JPEG_CS_Y709) {
+                return -1;
+        }
+        return decode(d, stream, len, dst, dst_is_device, dst_pitch, out_codec, rshift, gshift, bshift, stream_cs, out_cs, true);
 }
 
 }  // extern "C"
