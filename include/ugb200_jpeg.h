@@ -176,7 +176,8 @@ UGB_API int ugb200_jpeg_decode(ugb200_jpeg_decoder *dec, const uint8_t *stream, 
  *   UGB200_JPEG_CS_NATIVE: the bytes of ugb200_jpeg_decode.
  *   UGB200_JPEG_CS_Y709 | _Y601 | _Y601FULL: what the stream's YCbCr holds.  R = clamp((y_scale * (Y - o) + r_cr * (Cr - 128)) >> 14, 0, 255), G and B
  *     likewise (UltraGrid's YCBCR_TO_R/G/B) with the coefficients coeffs_709(8), coeffs_601(8), coeffs_601(0) of UltraGrid's color_space.c, o = 16,
- *     16, 0, and >> a floor.  Chroma is replicated from its pixel pair (4:2:2) or quad (4:2:0), not interpolated.  RGBA places R, G and B at the
+ *     16, 0, and >> a floor.  Chroma is replicated from its pixel pair (4:2:2) or quad (4:2:0) unless the decoder interpolates it
+ *     (ugb200_jpeg_decoder_set_upsampling).  RGBA places R, G and B at the
  *     shifts and sets every other bit (alpha 0xFF).  Y709 RGB output of a 4:2:2 or 4:2:0 stream is the RGB of ugb200_jpeg_decode byte for byte.
  *   UGB200_JPEG_CS_AUTO: as ugb200_jpeg_stream_color_space resolves it; a stream that declares RGB is not transformed, a refusal is returned.
  * RGB and four-component streams, and UYVY, I420 and VUYA output, keep the stream's samples in every mode (ugb200_jpeg_decode_to converts those).
@@ -211,6 +212,28 @@ UGB_API int ugb200_jpeg_decode_cs(ugb200_jpeg_decoder *dec, const uint8_t *strea
  * Errors as ugb200_jpeg_decode_cs; on every error the output buffer is not touched. */
 UGB_API int ugb200_jpeg_decode_to(ugb200_jpeg_decoder *dec, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch,
                                   int out_codec, int rshift, int gshift, int bshift, int stream_cs, int out_cs);
+
+/* Chroma upsampling of RGB and RGBA output in a colour space.  REPLICATE (the default) gives every pixel the chroma of its pair or quad, as above.
+ * FANCY interpolates it as libjpeg-turbo (and so every libjpeg- or ffmpeg-based viewer) does, so that saturated edges show no 2-pixel colour steps.
+ * FANCY changes only RGB and RGBA output of a 4:2:2 or 4:2:0 YCbCr stream from ugb200_jpeg_decode_cs and ugb200_jpeg_decode_to, and only when the
+ * colour space is Y709, Y601 or Y601FULL, or AUTO resolving to one of them.  For those outputs:
+ *   1. Each chroma plane (Cb, Cr) is upsampled to full resolution with integers and `>>` a floor.  The plane has cw = ceil(w / 2) columns and
+ *      ch = h rows (4:2:2) or ceil(h / 2) rows (4:2:0); a neighbour outside [0, cw - 1] x [0, ch - 1] takes the value of the nearest edge sample, so
+ *      the padded block area beyond cw / ch is never read.
+ *        4:2:2, chroma sample c[x] of a row:  out[2x] = (3 c[x] + c[x-1] + 1) >> 2,  out[2x+1] = (3 c[x] + c[x+1] + 2) >> 2
+ *        4:2:0, chroma rows c (this row) and n (the row above for output row 2y, the row below for 2y + 1), s[x] = 3 c[x] + n[x]:
+ *                                             out[2x] = (3 s[x] + s[x-1] + 8) >> 4,  out[2x+1] = (3 s[x] + s[x+1] + 7) >> 4
+ *      When cw <= 2 the chroma is replicated instead, in both directions, as libjpeg-turbo does for planes that narrow (jdsample.c).  Output
+ *      columns and rows past w / h are dropped.
+ *   2. Every pixel then gets YCBCR_TO_R/G/B of ugb200_jpeg_decode_cs with its own luma and its own upsampled Cb, Cr, clamped 0..255; RGBA as there.
+ *   3. Every pixel of every row is written, w * 3 or w * 4 bytes and nothing beyond - the last pixel of an odd width included, which REPLICATE
+ *      leaves unwritten.
+ * Byte for byte the same under FANCY as under REPLICATE: ugb200_jpeg_decode, colour space NATIVE, UYVY / I420 / VUYA output, 4:4:4, grayscale, RGB
+ * and four-component streams, AUTO resolving to RGB, and every refusal.  The filter and its edge rule equal libjpeg-turbo's YCbCr output sample for
+ * sample (tests/test_jpeg_decode_fancy.py).
+ * mode applies to every later decode call on this decoder.  0 ok, -1 bad arguments (NULL decoder, unknown mode). */
+enum { UGB200_JPEG_UPSAMPLE_REPLICATE = 0, UGB200_JPEG_UPSAMPLE_FANCY = 1 };
+UGB_API int ugb200_jpeg_decoder_set_upsampling(ugb200_jpeg_decoder *dec, int mode);
 
 #ifdef __cplusplus
 }

@@ -180,6 +180,24 @@ if ONLY != "staged":
                         assert is444 and out_c == 1 and cs_in == "native"
                     n += 1
     dec5.close()
+# JPEG decode with interpolated chroma (ugb200_jpeg_decoder_set_upsampling FANCY): the halo IDCT and the filter phase of the fused kernel, 4:2:2 and
+# 4:2:0 at odd and even sizes down to 1 x 1 and widths across CTA boundaries (512 pixels), to RGB and RGBA, tight and pitched device destinations
+if ONLY != "staged":
+    dec6 = api.JpegDecoder()
+    dec6.set_upsampling("fancy")
+    for ss in (1, 2):
+        for w, h in ((1, 1), (2, 2), (3, 3), (5, 17), (64, 32), (333, 211), (513, 9), (1041, 40), (1553, 17)):
+            b = io.BytesIO()
+            Image.fromarray(natural_rgb(w, h, 6)).save(b, "JPEG", quality=90, subsampling=ss)
+            s = b.getvalue()
+            for out_c in (12, 1):  # RGB, RGBA
+                ls = vc_get_linesize(w, out_c)
+                for pitch in (ls, ls + 40):
+                    for cs in ("Y709", "Y601", "Y601full", "auto"):
+                        out = torch.empty(pitch * h, dtype=torch.uint8, device="cuda")
+                        dec6.decode(s, out_c, shifts=(8, 16, 0) if out_c == 1 else (0, 8, 16), device=True, pitch=pitch, out=out, color_space=cs)
+                        n += 1
+    dec6.close()
 # LDGM FEC: encode from host (packets of 4-, 8- and 16-byte words) and from a device frame at offsets 4 and 1 into a tight device buffer;
 # decode with losses peeling can repair (several levels) and with losses it cannot
 import ldgm_cases as lc

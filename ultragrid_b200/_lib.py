@@ -107,6 +107,7 @@ SIGNATURES = {
     "ugb200_jpeg_decoder_create": (_vp, [_vp]),
     "ugb200_jpeg_decoder_destroy": (None, [_vp]),
     "ugb200_jpeg_decoder_expect": (_i, [_vp, _i, _i]),
+    "ugb200_jpeg_decoder_set_upsampling": (_i, [_vp, _i]),
     "ugb200_jpeg_decode": (_i, [_vp, _vp, _sz, _vp, _i, _l, _i, _i, _i, _i]),
     "ugb200_jpeg_decode_cs": (_i, [_vp, _vp, _sz, _vp, _i, _l, _i, _i, _i, _i, _i]),
     "ugb200_jpeg_decode_to": (_i, [_vp, _vp, _sz, _vp, _i, _l, _i, _i, _i, _i, _i, _i]),

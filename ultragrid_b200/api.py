@@ -368,6 +368,12 @@ class JpegDecoder:
         _check(_L.ugb200_jpeg_decoder_last_sync(self._h, ctypes.byref(st)), "ugb200_jpeg_decoder_last_sync")
         return {"scans": st.scans, "subsequences": st.subsequences, "rounds": st.rounds}
 
+    def set_upsampling(self, mode):
+        """ugb200_jpeg_decoder_set_upsampling: chroma of RGB / RGBA output in a colour space, ``"replicate"`` (the default) or ``"fancy"``
+        (libjpeg's interpolation; 4:2:2 and 4:2:0 streams), or its value, for every later decode"""
+        m = JPEG_UPSAMPLE[mode] if isinstance(mode, str) else int(mode)
+        _check(_L.ugb200_jpeg_decoder_set_upsampling(self._h, m), "ugb200_jpeg_decoder_set_upsampling")
+
     def decode(self, stream, out_codec, shifts=(0, 8, 16), device=False, pitch=0, out=None, sync=True, color_space=None, out_cs=None):
         """bytes -> numpy array (host) or CUDA tensor (device=True) holding height rows of vc_get_linesize(width, out_codec) bytes.
         ``color_space`` None: ugb200_jpeg_decode (the stream's samples, RGB / RGBA through UltraGrid's line converters); else one of
@@ -412,6 +418,8 @@ class JpegDecoder:
 
 # UGB200_JPEG_CS_* of include/ugb200_jpeg.h
 JPEG_CS = {"native": 0, "Y601": 1, "Y601full": 2, "Y709": 3, "RGB": 4, "auto": 5}
+# UGB200_JPEG_UPSAMPLE_*
+JPEG_UPSAMPLE = {"replicate": 0, "fancy": 1}
 
 
 def jpeg_stream_color_space(stream):

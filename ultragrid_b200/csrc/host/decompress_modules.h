@@ -52,6 +52,29 @@ static int jpeg_decode_cs_from_env()
         fprintf(stderr, "[GPUJPEG dec.] UGB200_JPEG_DECODE_CS=%s is not one of auto, y709, y601, y601full: ignored\n", e);
         return UGB200_JPEG_CS_NATIVE;
 }
+/// The chroma upsampling of the JPEG modules' RGB / RGBA output, read when a module instance is created next to UGB200_JPEG_DECODE_CS:
+/// UGB200_JPEG_DECODE_UPSAMPLE=fancy|replicate (ugb200_jpeg_decoder_set_upsampling).  It acts only together with a colour space, because FANCY changes
+/// nothing of the native bytes; unset, the chroma is replicated as before.
+static int jpeg_decode_upsample_from_env(int stream_cs)
+{
+        const char *e = getenv("UGB200_JPEG_DECODE_UPSAMPLE");
+        if (e == nullptr || e[0] == 0) {
+                return UGB200_JPEG_UPSAMPLE_REPLICATE;
+        }
+        int mode;
+        if (strcmp(e, "fancy") == 0) {
+                mode = UGB200_JPEG_UPSAMPLE_FANCY;
+        } else if (strcmp(e, "replicate") == 0) {
+                mode = UGB200_JPEG_UPSAMPLE_REPLICATE;
+        } else {
+                fprintf(stderr, "[GPUJPEG dec.] UGB200_JPEG_DECODE_UPSAMPLE=%s is not one of fancy, replicate: ignored\n", e);
+                return UGB200_JPEG_UPSAMPLE_REPLICATE;
+        }
+        if (stream_cs == UGB200_JPEG_CS_NATIVE) {
+                fprintf(stderr, "[GPUJPEG dec.] note: UGB200_JPEG_DECODE_UPSAMPLE=%s has an effect only together with UGB200_JPEG_DECODE_CS\n", e);
+        }
+        return mode;
+}
 /// ugb200_jpeg_decode_to with the module's colour space: NATIVE gives the bytes of ugb200_jpeg_decode (and decodes grayscale streams, which that call refuses)
 static int jpeg_module_decode(ugb200_jpeg_decoder *dec, int stream_cs, const unsigned char *buffer, size_t len, void *dst, int dst_is_device, long pitch, int out_codec,
                               int rshift, int gshift, int bshift)
@@ -69,6 +92,7 @@ struct state_decompress_gpujpeg {  // gpujpeg.c:63-70
         int rshift = 0, gshift = 0, bshift = 0, pitch = 0;
         codec_t out_codec = VIDEO_CODEC_NONE;
         int stream_cs = jpeg_decode_cs_from_env();
+        int upsampling = jpeg_decode_upsample_from_env(stream_cs);
 };
 }  // namespace
 
@@ -89,6 +113,9 @@ static int gpujpeg_decompress_reconfigure(void *state, struct video_desc desc, i
         s->desc = desc, s->rshift = rshift, s->gshift = gshift, s->bshift = bshift, s->pitch = pitch, s->out_codec = out_codec;
         if (!s->decoder) {
                 s->decoder = ugb200_jpeg_decoder_create(nullptr);
+                if (s->decoder) {
+                        ugb200_jpeg_decoder_set_upsampling(s->decoder, s->upsampling);
+                }
         }
         // dst holds pitch * desc.height bytes: a stream that declares another size must not be decoded into it
         return s->decoder != nullptr && ugb200_jpeg_decoder_expect(s->decoder, (int) desc.width, (int) desc.height) == 0;
@@ -147,6 +174,7 @@ struct state_gpujpeg_to_dxt {
         void *rgb = nullptr, *dxt = nullptr;  // device
         size_t rgb_cap = 0, dxt_cap = 0;
         int stream_cs = jpeg_decode_cs_from_env();
+        int upsampling = jpeg_decode_upsample_from_env(stream_cs);
         struct video_desc desc{};
         codec_t out_codec = VIDEO_CODEC_NONE;
 };
@@ -162,6 +190,7 @@ static void *gpujpeg_to_dxt_init(void)
                 delete s;
                 return nullptr;
         }
+        ugb200_jpeg_decoder_set_upsampling(s->decoder, s->upsampling);
         return s;
 }
 static int gpujpeg_to_dxt_reconfigure(void *state, struct video_desc desc, int, int, int, int pitch, codec_t out_codec)

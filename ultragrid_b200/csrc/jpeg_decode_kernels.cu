@@ -16,7 +16,9 @@
 //                           oracle/jpeg_decode_oracle.c), level shift, clamp, 8 x 8-byte stores into the component plane
 //   K2'    jpeg_idct_packed_kernel  instead of K2 for 4:2:2 and 4:2:0 YCbCr: the IDCT of an MCU row's blocks into a shared tile, chroma replicated
 //                           from its pair or quad, and the UYVY words stored as UYVY or handed to a line converter functor (yuv_rgb_conv.cuh):
-//                           UltraGrid's UYVY -> RGB / RGBA, or the integer YCbCr -> RGB of a colour space (ugb200_jpeg_decode_cs); no planes
+//                           UltraGrid's UYVY -> RGB / RGBA, or the integer YCbCr -> RGB of a colour space (ugb200_jpeg_decode_cs); no planes.
+//                           With ugb200_jpeg_decoder_set_upsampling(FANCY), RGB / RGBA in a colour space: libjpeg's interpolated chroma instead
+//                           (epi_fancy; the halo of neighbouring chroma blocks is IDCT'd in the kernel)
 //   pack   the component planes of K2 go through the from_planar kernels that already exist (planar_conv_kernels.cu): 4:4:4 YCbCr -> VUYA
 //                           (yuv444p_to_vuya), RGB -> RGB (rgbpXX_to_rgb), R G B A (gbrap_to_rgba); then ugb200_pixfmt_convert when another
 //                           output codec was asked for (also from K2's UYVY to VUYA / I420).  4:4:4 YCbCr in a colour space: jpeg_planes_cs_kernel.
@@ -612,6 +614,167 @@ using epi_cs_rgb = epi_conv<conv_yuv422_rgb<1, 3, 0, 2, CS>>;
 template <class CS>
 using epi_cs_rgba = epi_conv<conv_yuv422_rgb<1, 3, 0, 2, CS, true>>;
 
+/// RGB / RGBA output in a colour space with libjpeg's interpolated chroma (UGB200_JPEG_UPSAMPLE_FANCY): every pixel of the row, 16 per thread,
+/// YCBCR_TO_R/G/B of its own luma and its own upsampled Cb, Cr (the integers of jpeg_planes_cs_kernel); staged like epi_conv
+template <class CS, bool RGBA>
+struct epi_fancy {
+        static constexpr int PX = 16, BPP = RGBA ? 4 : 3, OUT = 16 * BPP;
+        using cs = CS;
+        static constexpr bool rgba = RGBA;
+};
+template <class E>
+constexpr bool is_fancy = false;
+template <class CS, bool RGBA>
+constexpr bool is_fancy<epi_fancy<CS, RGBA>> = true;
+
+/// FANCY: both chroma tiles of the CTA with their halo, rows -1..8 of the MCU row (4:2:2: rows 0..7 only) x columns -1..256 (byte 7 = column -1,
+/// bytes 8..263 = the CTA's 256 columns, byte 264 = column 256; 16-byte rows)
+constexpr int kFancyRow = 272;
+__device__ __forceinline__ uint8_t (*fancy_chroma())[10][kFancyRow]
+{
+        __shared__ __align__(16) uint8_t s[2][10][kFancyRow];
+        return s;
+}
+
+/// dequantisation and column pass of one block, the arithmetic of jpeg_idct_packed_kernel
+__device__ __forceinline__ void idct_columns(const int16_t *__restrict__ blk, const float *mq, float *f)
+{
+        const uint4 *src = (const uint4 *) blk;
+#pragma unroll
+        for (int q = 0; q < 8; ++q) {
+                const uint4 v = __ldg(src + q);
+                const uint32_t w[4] = { v.x, v.y, v.z, v.w };
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                        const int lo = (int) (short) (w[j] & 0xffffu), hi = (int) w[j] >> 16;
+                        f[8 * q + 2 * j] = __fmul_rn(__fadd_rn(__uint_as_float(0x4B400000u + (uint32_t) lo), -12582912.0f), mq[8 * q + 2 * j]);
+                        f[8 * q + 2 * j + 1] = __fmul_rn(__fadd_rn(__uint_as_float(0x4B400000u + (uint32_t) hi), -12582912.0f), mq[8 * q + 2 * j + 1]);
+                }
+        }
+#pragma unroll
+        for (int col = 0; col < 8; ++col) {
+                idct8(f[col], f[8 + col], f[16 + col], f[24 + col], f[32 + col], f[40 + col], f[48 + col], f[56 + col]);
+        }
+}
+
+/// row pass of row r after idct_columns: the 8 samples as jpeg_idct_packed_kernel stores them in its tile
+__device__ __forceinline__ uint2 idct_row(const float *f, int r)
+{
+        float v[8];
+#pragma unroll
+        for (int x = 0; x < 8; ++x) {
+                v[x] = f[8 * r + x];
+        }
+        idct8(v[0], v[1], v[2], v[3], v[4], v[5], v[6], v[7]);
+        uint32_t o[8];
+#pragma unroll
+        for (int x = 0; x < 8; ++x) {
+                const int s = (int) __float_as_uint(__fadd_rn(__fadd_rn(v[x], 128.0f), 12582912.0f)) - 0x4B400000;
+                o[x] = (uint32_t) min(max(s, 0), 255);
+        }
+        return make_uint2(o[0] | o[1] << 8 | o[2] << 16 | o[3] << 24, o[4] | o[5] << 8 | o[6] << 16 | o[7] << 24);
+}
+
+/// FANCY: fill fancy_chroma() from the CTA's chroma tiles and the halo.  The halo is the IDCT of the neighbouring chroma blocks, computed here with
+/// the same operations as the CTA that owns them, so a halo sample equals that CTA's sample bit for bit: the last column of block mx0 - 1 and the
+/// first of block mx0 + 32 (full IDCT, one thread per block), and for 4:2:0 the last row of the 34 blocks mx0 - 1 .. mx0 + 32 of the MCU row above and
+/// the first row of those below (column pass and one row pass).  Blocks outside the grid are skipped: the clamp of fancy_rgb never reads them.
+template <int V>
+__device__ __forceinline__ void fancy_fill(const int16_t *__restrict__ coef, const float (*s_m)[64], const uint2 (*s_tile)[8][32], const dec_geom &g, int tid, int nt)
+{
+        uint8_t(*s_c)[10][kFancyRow] = fancy_chroma();
+        for (int i = tid; i < 512; i += nt) {
+                const int comp = i >> 8, r = (i >> 5) & 7, m = i & 31;
+                *(uint2 *) &s_c[comp][r + 1][8 + 8 * m] = s_tile[2 * V + comp][r][m];
+        }
+        const int mcux = g.c[1].bw, mcuy = g.c[1].bh, mx0 = blockIdx.x * 32, my = blockIdx.y;
+        constexpr int NROW = V == 2 ? 2 * 2 * 34 : 0;  // (component, above / below, block) tasks of the vertical halo
+        float f[64];
+        if (tid < NROW) {
+                const int comp = tid / 68, below = (tid / 34) & 1, X = mx0 - 1 + tid % 34, Y = below ? my + 1 : my - 1;
+                if (X >= 0 && X < mcux && Y >= 0 && Y < mcuy) {
+                        const dec_comp &c = g.c[1 + comp];
+                        idct_columns(coef + ((long) c.blk_off + (long) Y * c.bw + X) * 64, s_m[c.tq], f);
+                        *(uint2 *) &s_c[comp][below ? 9 : 0][8 * (X - mx0 + 1)] = below ? idct_row(f, 0) : idct_row(f, 7);  // f stays in registers
+                }
+        } else if (tid < NROW + 4) {
+                const int t = tid - NROW, comp = t >> 1, right = t & 1, X = right ? mx0 + 32 : mx0 - 1;
+                if (X >= 0 && X < mcux) {
+                        const dec_comp &c = g.c[1 + comp];
+                        idct_columns(coef + ((long) c.blk_off + (long) my * c.bw + X) * 64, s_m[c.tq], f);
+#pragma unroll
+                        for (int r = 0; r < 8; ++r) {
+                                const uint2 v = idct_row(f, r);
+                                s_c[comp][r + 1][right ? 264 : 7] = (uint8_t) (right ? v.x : v.y >> 24);
+                        }
+                }
+        }
+}
+
+/// FANCY: the RGB / RGBA bytes of the 16 pixels of MCU `mcu` in pixel row `row` of the CTA.  Chroma is upsampled as libjpeg-turbo does it
+/// (jdsample.c h2v1 / h2v2 fancy upsampling): a neighbour outside [0, cw - 1] x [0, ch - 1] takes the nearest edge sample, and chroma rows of at most
+/// two samples are replicated, as libjpeg-turbo replicates them.
+template <int V, class CS, bool RGBA>
+__device__ __forceinline__ void fancy_rgb(const uint2 (*s_tile)[8][32], const dec_geom &g, int row, int mcu, uint32_t *o, const conv_params &p)
+{
+        const uint8_t(*s_c)[10][kFancyRow] = fancy_chroma();
+        const int cw = (g.w + 1) / 2, ch = V == 2 ? (g.h + 1) / 2 : g.h;
+        const int x0 = (blockIdx.x * 32 + mcu) * 8, base = 8 - (int) blockIdx.x * 256;  // byte of global chroma column x: base + x
+        const int cr = V == 2 ? row >> 1 : row;
+        // 4:2:0: the tile row of the neighbouring chroma row (above for an even pixel row, below for an odd one)
+        const int nr = V == 2 ? min(max((int) blockIdx.y * 8 + cr + (row & 1 ? 1 : -1), 0), ch - 1) - (int) blockIdx.y * 8 + 1 : 0;
+        int up[2][16];
+#pragma unroll
+        for (int comp = 0; comp < 2; ++comp) {
+                if (cw <= 2) {
+#pragma unroll
+                        for (int j = 0; j < 8; ++j) {
+                                up[comp][2 * j] = up[comp][2 * j + 1] = s_c[comp][cr + 1][base + x0 + j];
+                        }
+                        continue;
+                }
+                int s[10];  // columns x0 - 1 .. x0 + 8, each clamped to [0, cw - 1]: c (4:2:2) or 3 c + n (4:2:0)
+#pragma unroll
+                for (int k = 0; k < 10; ++k) {
+                        const int x = base + min(max(x0 + k - 1, 0), cw - 1);
+                        const int c = s_c[comp][cr + 1][x];
+                        s[k] = V == 2 ? 3 * c + s_c[comp][nr][x] : c;
+                }
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                        if (V == 2) {
+                                up[comp][2 * j] = (3 * s[j + 1] + s[j] + 8) >> 4, up[comp][2 * j + 1] = (3 * s[j + 1] + s[j + 2] + 7) >> 4;
+                        } else {
+                                up[comp][2 * j] = (3 * s[j + 1] + s[j] + 1) >> 2, up[comp][2 * j + 1] = (3 * s[j + 1] + s[j + 2] + 2) >> 2;
+                        }
+                }
+        }
+        constexpr color_coeffs c = CS::coeffs();
+        const uint2 ya = s_tile[(V == 2 ? 2 * (row >> 3) : 0)][row & 7][mcu], yb = s_tile[(V == 2 ? 2 * (row >> 3) : 0) + 1][row & 7][mcu];
+        const uint32_t amask = 0xFFFFFFFFu ^ (0xFFu << p.rshift) ^ (0xFFu << p.gshift) ^ (0xFFu << p.bshift);
+        if (!RGBA) {
+#pragma unroll
+                for (int q = 0; q < 12; ++q) {
+                        o[q] = 0;
+                }
+        }
+#pragma unroll
+        for (int i = 0; i < 16; ++i) {
+                const uint32_t yw = i < 4 ? ya.x : i < 8 ? ya.y : i < 12 ? yb.x : yb.y;
+                const int ys = c.y_scale * ((int) ((yw >> (8 * (i & 3))) & 0xffu) - CS::y_off), cb = up[0][i] - 128, cr2 = up[1][i] - 128;
+                const uint32_t r = (uint32_t) min(max((ys + c.r_cr * cr2) >> COMP_BASE, 0), 255),
+                               gg = (uint32_t) min(max((ys + c.g_cb * cb + c.g_cr * cr2) >> COMP_BASE, 0), 255),
+                               b = (uint32_t) min(max((ys + c.b_cb * cb) >> COMP_BASE, 0), 255);
+                if (RGBA) {
+                        o[i] = amask | r << p.rshift | gg << p.gshift | b << p.bshift;
+                } else {
+                        o[(3 * i) >> 2] |= r << (8 * ((3 * i) & 3));
+                        o[(3 * i + 1) >> 2] |= gg << (8 * ((3 * i + 1) & 3));
+                        o[(3 * i + 2) >> 2] |= b << (8 * ((3 * i + 2) & 3));
+                }
+        }
+}
+
 /// the UYVY words of 8 pixels: 8 luma samples, the 4 Cb and 4 Cr samples of their pairs
 __device__ __forceinline__ void uyvy_words(uint2 Y, uint32_t C, uint32_t R, uint32_t *w)
 {
@@ -686,6 +849,10 @@ __global__ void __launch_bounds__(32 * (GRAY ? 2 : 2 * V + 2)) jpeg_idct_packed_
                 }
         }
         __syncthreads();
+        if constexpr (is_fancy<E>) {
+                fancy_fill<V>(coef, s_m, s_tile, g, tid, NT);
+                __syncthreads();
+        }
         if constexpr (MX) {
                 const int ybias = 8192 - ym.yy * ym.o_in;
                 auto conv4 = [&](uint32_t y, int t0, int t1) {  // four luma samples, two pairs
@@ -773,7 +940,7 @@ __global__ void __launch_bounds__(32 * (GRAY ? 2 : 2 * V + 2)) jpeg_idct_packed_
                 }
                 return;
         }
-        const int row_full = E::BPP == 2 ? ((g.w + 1) / 2) * 4 : (g.w / 2) * 2 * E::BPP;
+        const int row_full = is_fancy<E> ? g.w * E::BPP : E::BPP == 2 ? ((g.w + 1) / 2) * 4 : (g.w / 2) * 2 * E::BPP;
         for (int cidx = tid; cidx < ROWS * PPR; cidx += NT) {
                 const int row = cidx / PPR, piece = cidx % PPR, mcu = piece / (16 / E::PX), half = piece % (16 / E::PX);
                 const int y = my * ROWS + row;
@@ -781,21 +948,26 @@ __global__ void __launch_bounds__(32 * (GRAY ? 2 : 2 * V + 2)) jpeg_idct_packed_
                         break;
                 }
                 const int lim = E::BPP == 2 || y == g.h - 1 || row_full <= pitch ? row_full : (int) pitch;
-                const int cb = 2 * V, crow = V == 2 ? row >> 1 : row, yb = V == 2 ? 2 * (row >> 3) : 0, yrow = row & 7;
-                uint2 CB, CR;
-                if constexpr (GRAY) {
-                        CB = CR = make_uint2(0x80808080u, 0x80808080u);
+                uint32_t o[E::OUT / 4];
+                if constexpr (is_fancy<E>) {
+                        fancy_rgb<V, typename E::cs, E::rgba>(s_tile, g, row, mcu, o, p);
                 } else {
-                        CB = s_tile[cb][crow][mcu], CR = s_tile[cb + 1][crow][mcu];
+                        const int cb = 2 * V, crow = V == 2 ? row >> 1 : row, yb = V == 2 ? 2 * (row >> 3) : 0, yrow = row & 7;
+                        uint2 CB, CR;
+                        if constexpr (GRAY) {
+                                CB = CR = make_uint2(0x80808080u, 0x80808080u);
+                        } else {
+                                CB = s_tile[cb][crow][mcu], CR = s_tile[cb + 1][crow][mcu];
+                        }
+                        uint32_t w[E::PX / 2];
+                        if (E::PX == 8) {
+                                uyvy_words(s_tile[yb + half][yrow][mcu], half ? CB.y : CB.x, half ? CR.y : CR.x, w);
+                        } else {
+                                uyvy_words(s_tile[yb][yrow][mcu], CB.x, CR.x, w);
+                                uyvy_words(s_tile[yb + 1][yrow][mcu], CB.y, CR.y, w + 4);
+                        }
+                        E::run(w, o, p);
                 }
-                uint32_t w[E::PX / 2], o[E::OUT / 4];
-                if (E::PX == 8) {
-                        uyvy_words(s_tile[yb + half][yrow][mcu], half ? CB.y : CB.x, half ? CR.y : CR.x, w);
-                } else {
-                        uyvy_words(s_tile[yb][yrow][mcu], CB.x, CR.x, w);
-                        uyvy_words(s_tile[yb + 1][yrow][mcu], CB.y, CR.y, w + 4);
-                }
-                E::run(w, o, p);
                 uint8_t *d = out + (long) y * pitch;
                 if constexpr (!STAGED) {
                         const int xoff = (mx0 + mcu) * 32 + half * 16;
@@ -1166,6 +1338,7 @@ struct ugb200_jpeg_decoder {
         } hs[2];
         unsigned frame_no = 0;
         int expect_w = 0, expect_h = 0;  // ugb200_jpeg_decoder_expect: the destination was sized for these; 0 = unchecked
+        int upsampling = UGB200_JPEG_UPSAMPLE_REPLICATE;  // ugb200_jpeg_decoder_set_upsampling
         // host scratch that keeps its capacity from frame to frame
         std::vector<uint64_t> scan_part[8], markers;
         std::vector<uint32_t> seg_begin, seg_end;
@@ -1769,6 +1942,15 @@ UGB_API int ugb200_jpeg_decoder_expect(ugb200_jpeg_decoder *d, int width, int he
         return 0;
 }
 
+UGB_API int ugb200_jpeg_decoder_set_upsampling(ugb200_jpeg_decoder *d, int mode)
+{
+        if (!d || (mode != UGB200_JPEG_UPSAMPLE_REPLICATE && mode != UGB200_JPEG_UPSAMPLE_FANCY)) {
+                return -1;
+        }
+        d->upsampling = mode;
+        return 0;
+}
+
 /// ugb200_jpeg_decode, ugb200_jpeg_decode_cs and ugb200_jpeg_decode_to: color_space is one of NATIVE, Y601, Y601FULL, Y709, AUTO; out_cs (the space of
 /// UYVY, I420 and VUYA output) one of NATIVE, Y601, Y601FULL, Y709; gray_ok: one-component streams are decoded (ugb200_jpeg_decode_to), else -4 as ever
 static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, void *dst, int dst_is_device, long dst_pitch, int out_codec, int rshift, int gshift,
@@ -2102,6 +2284,8 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
                 const dim3 grid((unsigned) (((gray ? (g.c[0].bw + 1) / 2 : g.c[1].bw) + 31) / 32), (unsigned) (gray ? g.c[0].bh : g.c[1].bh));
                 const bool vec = !(15 & (size_t) o) && !(op & 15);
                 const int kind = planar ? 8 : uyvy_out ? 0 : out_codec == UGB_RGB ? (conv_cs == UGB200_JPEG_CS_NATIVE ? UGB200_JPEG_CS_Y709 : conv_cs) : 4 + conv_cs;
+                // interpolated chroma (ugb200_jpeg_decoder_set_upsampling): RGB / RGBA of a 4:2:2 or 4:2:0 stream in a colour space only
+                const bool fancy = d->upsampling == UGB200_JPEG_UPSAMPLE_FANCY && !gray && conv_cs != UGB200_JPEG_CS_NATIVE;
                 auto launch = [&](auto v, auto gr) {
                         constexpr int V = decltype(v)::value;
                         constexpr bool G = decltype(gr)::value;
@@ -2110,6 +2294,19 @@ static int decode(ugb200_jpeg_decoder *d, const uint8_t *stream, size_t len, voi
                                 jpeg_idct_packed_kernel<V, typename decltype(e)::type, decltype(m)::value, G><<<grid, NT, 0, s>>>(d->coef, d->d_tables, g, o, op, vec, cp, ym);
                         };
                         const std::false_type plain;
+                        if constexpr (!G) {
+                                if (fancy) {
+                                        switch (kind) {
+                                        case UGB200_JPEG_CS_Y709: run(type_tag<epi_fancy<ycbcr_709, false>>(), plain); break;
+                                        case UGB200_JPEG_CS_Y601: run(type_tag<epi_fancy<ycbcr_601, false>>(), plain); break;
+                                        case UGB200_JPEG_CS_Y601FULL: run(type_tag<epi_fancy<ycbcr_601_full, false>>(), plain); break;
+                                        case 4 + UGB200_JPEG_CS_Y709: run(type_tag<epi_fancy<ycbcr_709, true>>(), plain); break;
+                                        case 4 + UGB200_JPEG_CS_Y601: run(type_tag<epi_fancy<ycbcr_601, true>>(), plain); break;
+                                        default: run(type_tag<epi_fancy<ycbcr_601_full, true>>(), plain); break;
+                                        }
+                                        return;
+                                }
+                        }
                         switch (kind) {
                         case 0: matrix ? run(type_tag<epi_uyvy>(), std::true_type()) : run(type_tag<epi_uyvy>(), plain); break;
                         case UGB200_JPEG_CS_Y709: run(type_tag<epi_rgb>(), plain); break;
