@@ -10,10 +10,10 @@
  * (to_lavc_vid_conv.c:115-128) - plane pointers and line sizes - and the pixel format by the enum below (INTEGRATION.md shows the
  * AV_PIX_FMT_* switch of the binding).  Pointers are DEVICE pointers (the planes are what an NVENC / hardware frame context consumes).
  *
- * PARITY: to_lavc_vid_conv.c cannot be compiled here (libavutil / libavcodec headers absent), so these kernels are pinned against
- * oracle/lavc_oracle.c, a restatement citing the reference lines, plus what the tree does allow: the colour coefficients against the reference build,
- * the conversions that delegate to src/to_planar.c against its unmodified objects, and the v210 <-> planar identities of
- * test/ff_codec_conversions_test.cpp:346-401. */
+ * PARITY: to_lavc_vid_conv.c and from_lavc_vid_conv.c cannot be compiled here (libavutil / libavcodec headers absent), so this bridge is NOT
+ * pinned against lavc itself.  tests/test_lavc_exact.py pins every pair it admits to a numpy restatement of the cited reference lines, and pins that
+ * restatement to what the tree does allow: the colour coefficients against the reference build, identities through the unmodified to_planar.c /
+ * from_planar.c objects (the idea of test/ff_codec_conversions_test.cpp:346-401), a bound of the float64 BT.709 matrix, and oracle/lavc_oracle.c. */
 #ifndef UGB200_LAVC_H
 #define UGB200_LAVC_H
 #include "ugb200.h"
@@ -44,8 +44,9 @@ struct ugb200_av_planes {        /* AVFrame::data / AVFrame::linesize */
 /* Is there a device conversion for this pair (the role of get_uv_to_av_conversions(), to_lavc_vid_conv.c:1458)? */
 UGB_API int ugb200_to_lavc_supported(int in_codec, int av_pixfmt);
 /* One frame: `in_data` = device frame of `in_codec`, rows vc_get_linesize(width, in_codec) apart, -> planes.  Asynchronous on `stream`.
- * 0 ok, -1 bad arguments / unsupported pair, -2 launch failure.  Loop bounds as the reference functions (whole v210 groups of 6, R12L
- * groups of 8 ...), except that no sample is written beyond a plane row's linesize. */
+ * 0 ok, -1 bad arguments / unsupported pair / a 16-bit plane at an odd address or line size / a v210 source that is not 4-byte aligned (the
+ * reference asserts both; nothing is written), -2 launch failure.  Loop bounds as the reference functions (whole v210 groups of 6, R12L groups
+ * of 8, UYVY pixel pairs ...), except that no sample is written beyond a plane row's linesize. */
 UGB_API int ugb200_to_lavc_convert(int in_codec, int av_pixfmt, const struct ugb200_av_planes *out, const void *in_data, int width, int height,
                                    cuda_wrapper_stream_t stream);
 

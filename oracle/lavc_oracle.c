@@ -57,7 +57,7 @@ API void orc_lavc_v210(int mode, const uint8_t *in, int width, int height, uint8
 API void orc_lavc_uyvy(int to444, const uint8_t *in, int width, int height, uint8_t *const p[3], const int ls[3])
 {
         for (int y = 0; y < height; ++y) {
-                const uint8_t *src = in + (long) y * width * 2;
+                const uint8_t *src = in + (long) y * ((width + 1) / 2) * 4; /* the source pointer runs on over (width + 1) / 2 pairs per row */
                 uint8_t *dy = p[0] + (long) ls[0] * y, *dcb = p[1] + (long) ls[1] * y, *dcr = p[2] + (long) ls[2] * y;
                 for (int x = 0; x < width; x += 2) {
                         *dcb++ = src[0];
@@ -98,7 +98,7 @@ API void orc_lavc_rgb(int src_kind, int depth, int sub422, const struct coeffs *
                 }
                 uint16_t *dy = (uint16_t *) (p[0] + (long) ls[0] * y), *dcb = (uint16_t *) (p[1] + (long) ls[1] * y), *dcr = (uint16_t *) (p[2] + (long) ls[2] * y);
                 if (src_kind == 0) {
-                        const uint8_t *s = in + (long) y * width * 4;
+                        const uint8_t *s = in + (long) y * ((width + 63) / 64) * 256; /* vc_get_linesize(width, R10k): 64-pixel rows (:712) */
                         for (int x = 0; x < width; ++x, s += 4) {
                                 put3(c, 10, depth, s[0] << 2 | s[1] >> 6, (s[1] & 0x3F) << 4 | s[2] >> 4, (s[2] & 0x0F) << 6 | s[3] >> 2, &Y, &CB, &CR);
                                 *dy++ = (uint16_t) Y, *dcb++ = (uint16_t) CB, *dcr++ = (uint16_t) CR;

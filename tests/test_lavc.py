@@ -1,6 +1,8 @@
-"""libavcodec bridge conversions (SURVEY.md section 8f rank 3; include/ugb200_lavc.h).  The reference file cannot be compiled here (FFmpeg headers
-absent) - PARITY UNPINNED against it; CPU part: the restatement oracle/lavc_oracle.c against what the tree does pin (colour coefficients of the
-unmodified color_space.c, identities through the unmodified to_planar.c / from_planar.c); GPU part: kernels == restatement, byte for byte."""
+"""libavcodec bridge conversions (SURVEY.md section 8f rank 3; include/ugb200_lavc.h).  CPU part: the restatement oracle/lavc_oracle.c against what
+the tree does pin (colour coefficients of the unmodified color_space.c, identities through the unmodified to_planar.c / from_planar.c); GPU part:
+kernels == restatement, byte for byte.  tests/test_lavc_exact.py pins every pair the library admits, in both directions, to a numpy restatement of
+the reference lines with no C oracle in between.  Still not pinned: the bridge against libavcodec itself (the reference's to_lavc_vid_conv.c and
+from_lavc_vid_conv.c need FFmpeg headers, which are not part of the tree)."""
 import ctypes
 
 import numpy as np
@@ -124,15 +126,18 @@ def test_gpu_to_lavc_equals_restatement(orc, ref_cpu, inc, fmt):
 
 @pytest.mark.gpu
 def test_gpu_delegated_conversions_equal_to_planar(orc):
-    """v210 -> P010LE, UYVY -> NV12 / YUV420P go through the to_planar kernels (as the reference delegates, to_lavc_vid_conv.c:132-135,186-189)"""
+    """v210 -> P010LE, Y216 -> P010LE and UYVY -> NV12 / YUV420P go through the to_planar kernels (as the reference delegates, to_lavc_vid_conv.c:132-135,
+    192-195) and equal the CPU restatement of to_planar.c (oracle/planar_oracle.c, pinned to the unmodified objects by test_planar.py)"""
     import torch
     from ultragrid_b200 import api
+    import test_lavc_exact as tle
     w, h = 96, 8
-    src = util.v210_noise(w, h, 9)
-    y, c = api.to_lavc(V210, "P010LE", torch.from_numpy(src).cuda(), w, h)
-    wy, wc = np.zeros(w * 2 * h, np.uint8), np.zeros(w * h, np.uint8)
-    orc.orc_v210_to_p010le(w, h, wy.ctypes.data, w * 2, wc.ctypes.data, w * 2, src.ctypes.data)
-    assert np.array_equal(y.cpu().numpy(), wy) and np.array_equal(c.cpu().numpy(), wc)
+    for inc, fmt in tle.DELEGATED:
+        src = tle.make_source(inc, w, h, 9)
+        got = api.to_lavc(inc, fmt, torch.from_numpy(src).cuda(), w, h)
+        want = tle.ref_to_lavc(inc, fmt, src, w, h, [ls for ls, _ in api.av_plane_shapes(fmt, w, h)], orc)
+        for i, (g, b, wr) in enumerate(zip(got, want.buf, want.wr)):
+            assert wr.all() and np.array_equal(g.cpu().numpy(), b.reshape(-1)), (inc, fmt, i)
 
 
 @pytest.mark.gpu

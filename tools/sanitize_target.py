@@ -219,5 +219,24 @@ for k, m, c in ([] if ONLY in ("jpeg", "staged") else ((64, 64, 2), (512, 384, 5
             coder.decode(buf, lc.packets_received(k + m, ps, rng.random(k + m) >= loss))
             n += 1
     coder.close()
+# libavcodec bridge: every to_lavc pair at odd sizes (v210 -> YUV420P10LE at odd height included) into tight, padded and odd-padded planes and into
+# planes 2 bytes into their buffers; every from_lavc pair the library accepts at odd sizes, with a tight and a wider pitch
+if ONLY not in ("jpeg", "staged"):
+    import test_lavc_exact as tle
+    L2, _ = tle.lib_and_torch()
+    for inc, fmt in tle.to_lavc_pairs():
+        for w, h in ((47, 5), (49, 3), (1, 1)):
+            src = tle.make_source(inc, w, h, 1)
+            for _, lss, off in tle.plane_modes(fmt, w, h):
+                assert tle.gpu_to_lavc(L2, torch, inc, fmt, src, w, h, lss, off)[0] == 0
+                n += 1
+    for fmt, outc in tle.from_lavc_pairs():
+        for w, h in ((47, 5), (15, 3)):
+            pl = tle.av_planes_in(fmt, w, h, 2, pad=3)
+            planes = [torch.from_numpy(a.reshape(-1).copy()).cuda() for a, _ in pl]
+            for pitch in (vc_get_linesize(w, outc), vc_get_linesize(w, outc) + 40):
+                dst = torch.zeros(pitch * h, dtype=torch.uint8, device="cuda")
+                api.from_lavc(fmt, outc, planes, [ls for _, ls in pl], w, h, dst, pitch)
+                n += 1
 torch.cuda.synchronize()
 print("exercised", n, "calls")

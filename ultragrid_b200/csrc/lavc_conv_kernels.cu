@@ -143,11 +143,22 @@ __global__ void __launch_bounds__(128) lavc_uyvy_kernel(const uint8_t *__restric
                                 *(uint32_t *) (dcr + x0 / 2) = v;
                         }
                 } else {
-                        for (int x = x0; x < min(x0 + 8, width); x += 2) {  // the reference steps two pixels at a time and writes both (:145-150)
+                        // the reference steps two pixels at a time and writes both (:145-150): an odd width writes one luma (4:4:4: and chroma)
+                        // sample more, kept only where the plane row has room for it
+                        for (int x = x0; x < min(x0 + 8, width); x += 2) {
                                 const uint8_t *p = in + (long) y * in_pitch + (long) x * 2;
-                                dy[x - x0] = p[1], dy[x - x0 + 1] = p[3];
+                                dy[x - x0] = p[1];
+                                if (x + 1 < o.ls[0]) {
+                                        dy[x - x0 + 1] = p[3];
+                                }
                                 if (TO444) {
-                                        dcb[x] = dcb[x + 1] = p[0], dcr[x] = dcr[x + 1] = p[2];
+                                        dcb[x] = p[0], dcr[x] = p[2];
+                                        if (x + 1 < o.ls[1]) {
+                                                dcb[x + 1] = p[0];
+                                        }
+                                        if (x + 1 < o.ls[2]) {
+                                                dcr[x + 1] = p[2];
+                                        }
                                 } else {
                                         dcb[x / 2] = p[0], dcr[x / 2] = p[2];
                                 }
@@ -341,6 +352,53 @@ __global__ void __launch_bounds__(256) lavc_gbrp_kernel(const uint8_t *__restric
         }
 }
 
+// ---- from_lavc YUV444P -> UYVY (from_lavc_vid_conv.c:663-685): width / 2 pixel pairs, chroma = (c[2x] + c[2x + 1]) / 2 (C truncation) ------------
+__global__ void __launch_bounds__(128) lavc_yuv444p_uyvy_kernel(const uint8_t *__restrict__ py, const uint8_t *__restrict__ pb,
+                                                                 const uint8_t *__restrict__ pr, long ls_y, long ls_b, long ls_r, uint8_t *out,
+                                                                 long pitch, int pairs, int height, bool al4)
+{
+        const int x = blockIdx.x * blockDim.x + threadIdx.x;
+        if (x >= pairs) {
+                return;
+        }
+        for (int y = blockIdx.y; y < height; y += gridDim.y) {
+                const uint8_t *sy = py + (long) y * ls_y + 2 * x, *sb = pb + (long) y * ls_b + 2 * x, *sr = pr + (long) y * ls_r + 2 * x;
+                const uint32_t u = ((uint32_t) __ldg(sb) + __ldg(sb + 1)) / 2, v = ((uint32_t) __ldg(sr) + __ldg(sr + 1)) / 2;
+                const uint32_t w = u | (uint32_t) __ldg(sy) << 8 | v << 16 | (uint32_t) __ldg(sy + 1) << 24;
+                uint8_t *d = out + (long) y * pitch + 4L * x;
+                if (al4) {
+                        *(uint32_t *) d = w;
+                } else {
+                        d[0] = (uint8_t) w, d[1] = (uint8_t) (w >> 8), d[2] = (uint8_t) (w >> 16), d[3] = (uint8_t) (w >> 24);
+                }
+        }
+}
+
+// ---- from_lavc YUV422P10LE -> v210 intermediate: the partial last 6-pixel group of each row, which yuv422p10le_to_v210 leaves out (from_planar.c:308)
+// and the line converter after it reads; samples beyond the width are 0 --------------------------------------------------------------------------
+__global__ void __launch_bounds__(128) lavc_v210_partial_kernel(const uint8_t *py, const uint8_t *pb, const uint8_t *pr, long ls_y, long ls_b,
+                                                                long ls_r, uint8_t *mid, long mid_pitch, int width, int height)
+{
+        const int y = blockIdx.x * blockDim.x + threadIdx.x;
+        if (y >= height) {
+                return;
+        }
+        const int g = width / 6, ny = width - 6 * g, nc = (width + 1) / 2 - 3 * g;
+        const uint16_t *sy = (const uint16_t *) (py + (long) y * ls_y) + 6 * g, *sb = (const uint16_t *) (pb + (long) y * ls_b) + 3 * g,
+                       *sr = (const uint16_t *) (pr + (long) y * ls_r) + 3 * g;
+        uint32_t Y[6], B[3], R[3];
+#pragma unroll
+        for (int i = 0; i < 6; ++i) {
+                Y[i] = i < ny ? sy[i] : 0u;
+        }
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+                B[i] = i < nc ? sb[i] : 0u, R[i] = i < nc ? sr[i] : 0u;
+        }
+        *(uint4 *) (mid + (long) y * mid_pitch + 16L * g) =
+                make_uint4(B[0] | Y[0] << 10 | R[0] << 20, Y[1] | B[1] << 10 | Y[2] << 20, R[1] | Y[3] << 10 | B[2] << 20, Y[4] | R[2] << 10 | Y[5] << 20);
+}
+
 struct lavc_fmt_info {
         int planes, depth_bytes, hsub, vsub;  // chroma subsampling shifts
         bool semi;                            // two-plane (NV12 / P010)
@@ -369,8 +427,8 @@ inline long linesize_of(int w, int codec)
 {
         switch (codec) {
         case UGB_v210: return (long) ((w + 47) / 48) * 128;
-        case UGB_UYVY: return (long) w * 2;
-        case UGB_R10k: return (long) w * 4;
+        case UGB_UYVY: return (long) ((w + 1) / 2) * 4;  // uyvy_to_yuv422p's source pointer runs on over (w + 1) / 2 pairs per row (:144)
+        case UGB_R10k: return (long) ((w + 63) / 64) * 256;  // vc_get_linesize: R10k rows are padded to 64 pixels (r10k_to_yuv444pXXle, :712)
         case UGB_RG48: return (long) w * 6;
         case UGB_R12L: return (long) ((w + 7) / 8) * 36;
         case UGB_RGB: return (long) w * 3;
@@ -415,6 +473,9 @@ int ugb200_to_lavc_convert(int in, int f, const struct ugb200_av_planes *out, co
         for (int i = 0; i < fi.planes; ++i) {
                 if (!out->data[i] || out->linesize[i] <= 0) {
                         return -1;
+                }
+                if (fi.depth_bytes == 2 && (((size_t) out->data[i] & 1) || (out->linesize[i] & 1))) {
+                        return -1;  // 16-bit samples: the reference asserts even line sizes (:200-202, :708-710, :763-765)
                 }
                 o.p[i] = out->data[i], o.ls[i] = out->linesize[i];
                 vec = vec && !((size_t) out->data[i] & 15) && !(out->linesize[i] & 15);
@@ -579,9 +640,24 @@ void ugb200_to_lavc_vid_conv_destroy(struct ugb200_to_lavc_conv **state)
 // ---- from_lavc: get_av_to_uv_cuda_conversion / av_to_uv_convert_cuda / av_to_uv_conversion_cuda_destroy (from_lavc_vid_conv_cuda.h:61-69) ----
 struct ugb200_av_to_uv_conv {
         int av_pixfmt, out_codec, mid_codec;  // planar stage produces mid_codec; a line converter follows when it differs from out_codec
-        void *d_mid;
-        size_t mid_cap;
+        void *d_mid, *d_out;  // intermediate frame; line-converter output when it writes whole groups past the destination's line
+        size_t mid_cap, out_cap;
 };
+
+static bool grow(void **p, size_t *cap, size_t need)
+{
+        if (need <= *cap) {
+                return true;
+        }
+        cudaFree(*p);
+        *p = nullptr, *cap = 0;
+        if (cudaMalloc(p, need) != cudaSuccess) {
+                *p = nullptr;
+                return false;
+        }
+        *cap = need;
+        return true;
+}
 
 static int planar_mid_codec(int av_pixfmt)
 {
@@ -603,20 +679,9 @@ struct ugb200_av_to_uv_conv *ugb200_get_av_to_uv_conversion(int av_pixfmt, int o
         }
         auto *s = new (std::nothrow) ugb200_av_to_uv_conv();
         if (s) {
-                s->av_pixfmt = av_pixfmt, s->out_codec = out_codec, s->mid_codec = mid, s->d_mid = nullptr, s->mid_cap = 0;
+                s->av_pixfmt = av_pixfmt, s->out_codec = out_codec, s->mid_codec = mid, s->d_mid = s->d_out = nullptr, s->mid_cap = s->out_cap = 0;
         }
         return s;
-}
-
-static long out_linesize(int w, int codec)
-{
-        switch (codec) {
-        case UGB_UYVY: return (long) w * 2;
-        case UGB_VUYA: return (long) w * 4;
-        case UGB_RGB: return (long) w * 3;
-        case UGB_v210: return (long) ((w + 47) / 48) * 128;
-        default: return 0;
-        }
 }
 
 int ugb200_av_to_uv_convert(struct ugb200_av_to_uv_conv *s, char *dst_buffer, const struct ugb200_av_planes *in, int width, int height, int pitch,
@@ -625,18 +690,37 @@ int ugb200_av_to_uv_convert(struct ugb200_av_to_uv_conv *s, char *dst_buffer, co
         if (!s || !dst_buffer || !in || width <= 0 || height <= 0) {
                 return -1;
         }
+        // the reference's own entries for YUV444P -> UYVY (yuv444p_to_uyvy, from_lavc_vid_conv.c:2100) and YUV422P10LE -> UYVY
+        // (yuv422p10le_to_uyvy, :2057) convert in one step; the VUYA / v210 intermediate would lose the second luma (vc_copylineVUYAtoUYVY takes
+        // it from the alpha byte, pixfmt_conv.c:2699) or the pixels of a partial 6-pixel group
+        if (s->out_codec == UGB_UYVY && (s->av_pixfmt == UGB_AV_YUV444P || s->av_pixfmt == UGB_AV_YUV422P10LE)) {
+                if (!in->data[0] || !in->data[1] || !in->data[2]) {
+                        return -1;
+                }
+                if (s->av_pixfmt == UGB_AV_YUV422P10LE) {
+                        struct ugb200_from_planar_data d{};
+                        d.width = width, d.height = height, d.out_data = (unsigned char *) dst_buffer, d.out_pitch = (unsigned) pitch, d.in_depth = 10;
+                        for (int i = 0; i < 3; ++i) {
+                                d.in_data[i] = in->data[i], d.in_linesize[i] = (unsigned) in->linesize[i];
+                        }
+                        return ugb200_yuv422p10le_to_uyvy(&d, stream);
+                }
+                const int pairs = width / 2;
+                if (pairs == 0) {
+                        return 0;
+                }
+                const dim3 grid((pairs + 127) / 128, min(height, 16384));
+                lavc_yuv444p_uyvy_kernel<<<grid, 128, 0, (cudaStream_t) stream>>>(in->data[0], in->data[1], in->data[2], in->linesize[0], in->linesize[1],
+                                                                                  in->linesize[2], (uint8_t *) dst_buffer, pitch, pairs, height,
+                                                                                  !((size_t) dst_buffer & 3) && !(pitch & 3));
+                return cudaGetLastError() == cudaSuccess ? 0 : -2;
+        }
         const bool direct = s->mid_codec == s->out_codec;
-        const long mid_pitch = direct ? pitch : out_linesize(width, s->mid_codec);
+        const long mid_pitch = direct ? pitch : (long) vc_get_linesize((unsigned) width, (codec_t) s->mid_codec);
         unsigned char *mid = (unsigned char *) dst_buffer;
         if (!direct) {
-                const size_t need = (size_t) mid_pitch * height + 64;
-                if (need > s->mid_cap) {
-                        cudaFree(s->d_mid);
-                        s->d_mid = nullptr, s->mid_cap = 0;
-                        if (cudaMalloc(&s->d_mid, need) != cudaSuccess) {
-                                return -2;
-                        }
-                        s->mid_cap = need;
+                if (!grow(&s->d_mid, &s->mid_cap, (size_t) mid_pitch * height + 64)) {
+                        return -2;
                 }
                 mid = (unsigned char *) s->d_mid;
         }
@@ -658,14 +742,36 @@ int ugb200_av_to_uv_convert(struct ugb200_av_to_uv_conv *s, char *dst_buffer, co
         if (rc != 0 || direct) {
                 return rc;
         }
-        return ugb200_pixfmt_convert(s->mid_codec, s->out_codec, dst_buffer, pitch, mid, mid_pitch, (int) vc_get_linesize((unsigned) width, (codec_t) s->out_codec), height,
-                                     (long) mid_pitch * height, d.rgb_shift[0], d.rgb_shift[1], d.rgb_shift[2], stream);
+        // A v210 intermediate: its partial last group is converted too, and the line converters after it write whole 6-pixel groups
+        // (vc_copylineV210toRGB, pixfmt_conv.c:2884-2940), past the destination's line when the width is not a multiple of 6.  They write into
+        // a frame of the rounded-up width, and the destination receives the lines.
+        const int wc = s->mid_codec == UGB_v210 ? (width + 5) / 6 * 6 : width;
+        const long ls = vc_get_linesize((unsigned) width, (codec_t) s->out_codec), lsc = vc_get_linesize((unsigned) wc, (codec_t) s->out_codec);
+        cudaStream_t st = (cudaStream_t) stream;
+        if (wc != width) {
+                lavc_v210_partial_kernel<<<(height + 127) / 128, 128, 0, st>>>(in->data[0], in->data[1], in->data[2], in->linesize[0], in->linesize[1],
+                                                                               in->linesize[2], mid, mid_pitch, width, height);
+        }
+        if (lsc == ls) {
+                return ugb200_pixfmt_convert(s->mid_codec, s->out_codec, dst_buffer, pitch, mid, mid_pitch, (int) ls, height, (long) mid_pitch * height,
+                                             d.rgb_shift[0], d.rgb_shift[1], d.rgb_shift[2], stream);
+        }
+        if (!grow(&s->d_out, &s->out_cap, (size_t) lsc * height + 64)) {
+                return -2;
+        }
+        rc = ugb200_pixfmt_convert(s->mid_codec, s->out_codec, s->d_out, lsc, mid, mid_pitch, (int) lsc, height, (long) mid_pitch * height, d.rgb_shift[0],
+                                   d.rgb_shift[1], d.rgb_shift[2], stream);
+        if (rc != 0) {
+                return rc;
+        }
+        return cudaMemcpy2DAsync(dst_buffer, pitch, s->d_out, lsc, ls, height, cudaMemcpyDeviceToDevice, st) == cudaSuccess ? 0 : -2;
 }
 
 void ugb200_av_to_uv_conversion_destroy(struct ugb200_av_to_uv_conv **state)
 {
         if (state && *state) {
                 cudaFree((*state)->d_mid);
+                cudaFree((*state)->d_out);
                 delete *state;
                 *state = nullptr;
         }

@@ -9,6 +9,7 @@
 // two rows above, to_planar.c:83-92,141-151 — note the reference's pointer arithmetic there is in uint16
 // elements, i.e. out_linesize *elements* = two rows up).
 #include <cuda_runtime.h>
+#include <limits.h>
 #include <stdint.h>
 
 #include "../../include/ugb200.h"
@@ -22,7 +23,7 @@ __device__ __forceinline__ uint32_t c2(uint32_t a0, uint32_t a1, uint32_t b0, ui
         return (((a0 + a1) / 2) << 6) | (((b0 + b1) / 2) << 22);
 }
 
-template <int G>  // groups per thread
+template <int G, bool SPILL>  // groups per thread; SPILL: a pair before the last writes whole groups past a row's end (see below)
 __global__ void __launch_bounds__(128) v210_to_p010_kernel(const uint8_t *__restrict__ in, long in_pitch, uint8_t *__restrict__ out_y,
                                                            long ls_y, uint8_t *__restrict__ out_c, long ls_c, int height,
                                                            int groups_mid, int groups_last, bool vec_ok)
@@ -74,7 +75,41 @@ __global__ void __launch_bounds__(128) v210_to_p010_kernel(const uint8_t *__rest
                 uint8_t *dy0 = out_y + (long) y * ls_y + (long) g0 * 12;
                 uint8_t *dy1 = dy0 + ls_y;
                 uint8_t *dc = out_c + (long) pr * ls_c + (long) g0 * 12;  // out_linesize[1] * y / 2, :79
-                if (full && vec_ok && G == 4) {
+                if (!SPILL) {  // every sample lands inside its own row
+                        if (full && vec_ok && G == 4) {
+#pragma unroll
+                                for (int i = 0; i < 3; ++i) {
+                                        ((uint4 *) dy0)[i] = make_uint4(oy0[4 * i], oy0[4 * i + 1], oy0[4 * i + 2], oy0[4 * i + 3]);
+                                        if (!single) {
+                                                ((uint4 *) dy1)[i] = make_uint4(oy1[4 * i], oy1[4 * i + 1], oy1[4 * i + 2], oy1[4 * i + 3]);
+                                        }
+                                        ((uint4 *) dc)[i] = make_uint4(oc[4 * i], oc[4 * i + 1], oc[4 * i + 2], oc[4 * i + 3]);
+                                }
+                        } else {
+#pragma unroll
+                                for (int i = 0; i < 3 * G; ++i) {
+                                        if (g0 + i / 3 < groups) {
+                                                // 2-byte granularity keeps this correct for any (even) out_linesize
+                                                ((uint16_t *) dy0)[2 * i] = (uint16_t) oy0[i], ((uint16_t *) dy0)[2 * i + 1] = (uint16_t) (oy0[i] >> 16);
+                                                if (!single) {
+                                                        ((uint16_t *) dy1)[2 * i] = (uint16_t) oy1[i], ((uint16_t *) dy1)[2 * i + 1] = (uint16_t) (oy1[i] >> 16);
+                                                }
+                                                ((uint16_t *) dc)[2 * i] = (uint16_t) oc[i], ((uint16_t *) dc)[2 * i + 1] = (uint16_t) (oc[i] >> 16);
+                                        }
+                                }
+                        }
+                        continue;
+                }
+                // A pair before the last converts (width + 5) / 6 groups (:89) and writes both rows group by group.  Past a tight row's end the
+                // first row's last samples land at the start of the second row after that row's own samples - they stay there - and the second
+                // row's land on the next pair's first row, which overwrites them later.  Pairs run concurrently here, so that order is made
+                // explicit: the first row keeps its whole groups, the second skips the samples the first row's spill owns and stops at its linesize.
+                // This holds when a row holds the width and the width at least one group (the spill, under 6 samples, then stays in the next
+                // row and comes from a later group than that row's own group 0); the host sends every other geometry to the serial kernel.
+                const long row = ls_y / 2, pos = (long) g0 * 6;  // samples per luma row; this thread's first sample
+                const long lim0 = last ? row : LONG_MAX, skip1 = last ? 0 : (long) groups * 6 - row;
+                const long lim1 = row, lim_c = ls_c / 2;
+                if (full && vec_ok && G == 4 && pos + 6 * G <= min(row, lim_c) && pos >= skip1) {
 #pragma unroll
                         for (int i = 0; i < 3; ++i) {
                                 ((uint4 *) dy0)[i] = make_uint4(oy0[4 * i], oy0[4 * i + 1], oy0[4 * i + 2], oy0[4 * i + 3]);
@@ -88,11 +123,18 @@ __global__ void __launch_bounds__(128) v210_to_p010_kernel(const uint8_t *__rest
                         for (int i = 0; i < 3 * G; ++i) {
                                 if (g0 + i / 3 < groups) {
                                         // 2-byte granularity keeps this correct for any (even) out_linesize
-                                        ((uint16_t *) dy0)[2 * i] = (uint16_t) oy0[i], ((uint16_t *) dy0)[2 * i + 1] = (uint16_t) (oy0[i] >> 16);
-                                        if (!single) {
-                                                ((uint16_t *) dy1)[2 * i] = (uint16_t) oy1[i], ((uint16_t *) dy1)[2 * i + 1] = (uint16_t) (oy1[i] >> 16);
+                                        for (int k = 0; k < 2; ++k) {
+                                                const long x = pos + 2 * i + k;
+                                                if (x < lim0) {
+                                                        ((uint16_t *) dy0)[2 * i + k] = (uint16_t) (oy0[i] >> (16 * k));
+                                                }
+                                                if (!single && x < lim1 && x >= skip1) {
+                                                        ((uint16_t *) dy1)[2 * i + k] = (uint16_t) (oy1[i] >> (16 * k));
+                                                }
+                                                if (x < lim_c) {
+                                                        ((uint16_t *) dc)[2 * i + k] = (uint16_t) (oc[i] >> (16 * k));
+                                                }
                                         }
-                                        ((uint16_t *) dc)[2 * i] = (uint16_t) oc[i], ((uint16_t *) dc)[2 * i + 1] = (uint16_t) (oc[i] >> 16);
                                 }
                         }
                 }
@@ -123,6 +165,56 @@ __global__ void v210_to_p010_tail_kernel(uint8_t *out_y, long ls_y, uint8_t *out
         }
 }
 
+/// The reference's loop itself (to_planar.c:73-152), in one thread, for the geometries the parallel kernel's ordering rule does not cover: a
+/// width below one group, where a pair's single group spills over several rows, or a plane row shorter than the width.  The final bytes are
+/// those of the reference's sequential writes; writes past the end of a plane (the reference's own overflow there) are dropped, and the tail
+/// copy that would read before the plane is skipped, as in v210_to_p010_tail_kernel.
+__global__ void v210_to_p010_serial_kernel(const uint8_t *__restrict__ in, long in_pitch, uint16_t *out_y, long ls_y, uint16_t *out_c, long ls_c,
+                                           int width, int height)
+{
+        const long ry = ls_y / 2, rc = ls_c / 2, ny = ry * height, nc = rc * ((height + 1) / 2);  // samples per row and per plane
+        for (int y = 0; y < height; y += 2) {
+                const bool single = height - y == 1, last = single || height - y == 2;  // :84-92
+                const uint32_t *a = (const uint32_t *) (in + (long) y * in_pitch), *b = single ? a : (const uint32_t *) (in + (long) (y + 1) * in_pitch);
+                long dy = (long) y * ry, dy2 = (long) (y + 1) * ry, dc = (long) (y / 2) * rc;
+                const int groups = last ? width / 6 : (width + 5) / 6;
+                for (int x = 0; x < groups; ++x, a += 4, b += 4) {
+                        const uint32_t ya[6] = { s10(a[0], 10), s10(a[1], 0), s10(a[1], 20), s10(a[2], 10), s10(a[3], 0), s10(a[3], 20) };
+                        const uint32_t yb[6] = { s10(b[0], 10), s10(b[1], 0), s10(b[1], 20), s10(b[2], 10), s10(b[3], 0), s10(b[3], 20) };
+                        const uint32_t c[6] = { (s10(a[0], 0) + s10(b[0], 0)) / 2,   (s10(a[0], 20) + s10(b[0], 20)) / 2, (s10(a[1], 10) + s10(b[1], 10)) / 2,
+                                                (s10(a[2], 0) + s10(b[2], 0)) / 2,   (s10(a[2], 20) + s10(b[2], 20)) / 2, (s10(a[3], 10) + s10(b[3], 10)) / 2 };
+                        for (int k = 0; k < 6; ++k, ++dy) {
+                                if (dy < ny) {
+                                        out_y[dy] = (uint16_t) (ya[k] << 6);
+                                }
+                        }
+                        for (int k = 0; k < 6 && !single; ++k, ++dy2) {  // a single last row writes its partner into a scratch row (:84-87)
+                                if (dy2 < ny) {
+                                        out_y[dy2] = (uint16_t) (yb[k] << 6);
+                                }
+                        }
+                        for (int k = 0; k < 6; ++k, ++dc) {
+                                if (dc < nc) {
+                                        out_c[dc] = (uint16_t) (c[k] << 6);
+                                }
+                        }
+                }
+                if (last && width % 6 != 0) {  // :141-151: pix_cnt samples from out_linesize ELEMENTS back, i.e. two rows up
+                        for (int i = 0; i < width % 6; ++i) {
+                                if (y >= 2 && dy + i < ny) {
+                                        out_y[dy + i] = out_y[dy - 2 * ry + i];
+                                }
+                                if (y >= 2 && height - y == 2 && dy2 + i < ny) {
+                                        out_y[dy2 + i] = out_y[dy - 2 * ry + i];
+                                }
+                                if (y / 2 >= 2 && dc + i < nc) {
+                                        out_c[dc + i] = out_c[dc - 2 * rc + i];
+                                }
+                        }
+                }
+        }
+}
+
 }  // namespace ugb
 
 extern "C" int ugb200_v210_to_p010le(const struct ugb200_to_planar_data *d, long in_linesize, cuda_wrapper_stream_t stream)
@@ -136,15 +228,28 @@ extern "C" int ugb200_v210_to_p010le(const struct ugb200_to_planar_data *d, long
                 in_linesize = (d->width + 47) / 48 * 128;  // vc_get_linesize(width, v210), video_codec.c:507-521
         }
         const int groups_mid = (d->width + 5) / 6, groups_last = d->width / 6;  // :89-92
+        cudaStream_t s = (cudaStream_t) stream;
+        if (d->width < 6 || d->out_linesize[0] / 2 < (unsigned) d->width || d->out_linesize[1] / 2 < (unsigned) d->width) {
+                v210_to_p010_serial_kernel<<<1, 1, 0, s>>>((const uint8_t *) d->in_data, in_linesize, (uint16_t *) d->out_data[0], d->out_linesize[0],
+                                                           (uint16_t *) d->out_data[1], d->out_linesize[1], d->width, d->height);
+                return cudaGetLastError() == cudaSuccess ? 0 : -2;
+        }
         const bool vec_ok = !(15 & (size_t) d->in_data) && !(in_linesize & 15) && !(15 & (size_t) d->out_data[0]) &&
                             !(15 & (size_t) d->out_data[1]) && !(d->out_linesize[0] & 15) && !(d->out_linesize[1] & 15);
         const int chunks = (groups_mid + 3) / 4, threads = 128;
         const int pairs = (d->height + 1) / 2;
         dim3 grid((chunks + threads - 1) / threads, pairs > 65535 ? 65535 : pairs);
-        cudaStream_t s = (cudaStream_t) stream;
-        v210_to_p010_kernel<4><<<grid, threads, 0, s>>>((const uint8_t *) d->in_data, in_linesize, (uint8_t *) d->out_data[0],
-                                                       d->out_linesize[0], (uint8_t *) d->out_data[1], d->out_linesize[1], d->height,
-                                                       groups_mid, groups_last, vec_ok);
+        // whole groups of a pair before the last reach past a row only when they are wider than it
+        const bool spill = d->height > 2 && (6L * groups_mid > d->out_linesize[0] / 2 || 6L * groups_mid > d->out_linesize[1] / 2);
+        if (spill) {
+                v210_to_p010_kernel<4, true><<<grid, threads, 0, s>>>((const uint8_t *) d->in_data, in_linesize, (uint8_t *) d->out_data[0],
+                                                                      d->out_linesize[0], (uint8_t *) d->out_data[1], d->out_linesize[1], d->height,
+                                                                      groups_mid, groups_last, vec_ok);
+        } else {
+                v210_to_p010_kernel<4, false><<<grid, threads, 0, s>>>((const uint8_t *) d->in_data, in_linesize, (uint8_t *) d->out_data[0],
+                                                                       d->out_linesize[0], (uint8_t *) d->out_data[1], d->out_linesize[1], d->height,
+                                                                       groups_mid, groups_last, vec_ok);
+        }
         const int pix_cnt = d->width % 6;
         if (pix_cnt != 0 && d->height > 2) {
                 v210_to_p010_tail_kernel<<<1, 32, 0, s>>>((uint8_t *) d->out_data[0], d->out_linesize[0], (uint8_t *) d->out_data[1],
