@@ -140,6 +140,26 @@ UGB_API int ugb200_yuv422pXX_to_uyvy(const struct ugb200_from_planar_data *d, cu
 UGB_API int ugb200_yuv422p10le_to_uyvy(const struct ugb200_from_planar_data *d, cuda_wrapper_stream_t stream);
 UGB_API int ugb200_yuv422p10le_to_v210(const struct ugb200_from_planar_data *d, cuda_wrapper_stream_t stream);  /* :295-333 (whole 6-pixel groups) */
 
+/* ---- interlaced video (src/video_codec.c, src/video_frame.c) ------------------------------------------ */
+/* vc_deinterlace_ex (video_codec.c:722-854): linear blend, out row y = (row y + row y+1 + 1) >> 1 per sample, then
+ * row lines-1 = out row lines-2 (src_linesize bytes).  Byte-exact on every byte the reference writes, in place
+ * (dst == src, dst_pitch == src_linesize) or out of place.  Differences (DESIGN.md §8): 16-bit codecs blend the
+ * whole row and R12L every whole 36-byte group, where the reference leaves the row's tail unwritten; opaque
+ * codecs are refused with -4.  lines == 1 copies the row for every non-opaque codec, as the reference does.
+ * -1: lines == 0, dst_pitch < src_linesize, partial overlap, or a 16-bit (word) codec at an address or pitch that
+ * is not a multiple of 2 (4).  -4: opaque codec, or DVS10 with lines > 1. */
+UGB_API int ugb200_vc_deinterlace_ex(int codec, const void *src, size_t src_linesize, void *dst, size_t dst_pitch, size_t lines,
+                                     cuda_wrapper_stream_t stream);
+/* vc_deinterlace (video_codec.c:597-711, the SSE2 form an x86-64 build runs): in-place recursive filter, any buffer
+ * address, byte-exact for linesize >= 16 (-1 below), including the last 16-byte column's re-filter of the next row's
+ * first bytes.  lines <= 4 leaves the buffer as it is. */
+UGB_API int ugb200_vc_deinterlace(void *buf, long linesize, int lines, cuda_wrapper_stream_t stream);
+/* il_upper_to_merged / il_merged_to_upper (video_frame.c:332-379): (height+1)/2 upper-field rows then height/2
+ * lower-field rows <-> interleaved rows.  dst == src works (stream-ordered scratch, no host wait); partial overlap
+ * is -1. */
+UGB_API int ugb200_il_upper_to_merged(void *dst, void *src, int linesize, int height, cuda_wrapper_stream_t stream);
+UGB_API int ugb200_il_merged_to_upper(void *dst, void *src, int linesize, int height, cuda_wrapper_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

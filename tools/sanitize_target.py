@@ -238,5 +238,27 @@ if ONLY not in ("jpeg", "staged"):
                 dst = torch.zeros(pitch * h, dtype=torch.uint8, device="cuda")
                 api.from_lavc(fmt, outc, planes, [ls for _, ls in pl], w, h, dst, pitch)
                 n += 1
+# interlaced video: vc_deinterlace_ex on tight buffers (dst ends at row lines-1's src_linesize), in place and out of place, lines 1-6, odd
+# line sizes, R12L's partial group and 16-bit rows that are not whole 16-byte chunks; vc_deinterlace at odd line sizes and addresses;
+# il_* in place and out of place
+if ONLY not in ("jpeg", "staged"):
+    for codec, ls in ((2, 3838), (2, 47), (7, 1004), (5, 68), (6, 36 * 5 + 8), (6, 8640), (27, 11508), (30, 20), (31, 14), (12, 5757)):
+        for lines in range(1, 7):
+            src = torch.randint(0, 256, (ls * lines,), dtype=torch.uint8, device="cuda")
+            dst = torch.zeros(ls * lines, dtype=torch.uint8, device="cuda")
+            api.deinterlace_ex(codec, src, ls, lines, dst=dst)
+            api.deinterlace_ex(codec, src, ls, lines, dst=src)
+            n += 2
+    for ls in (16, 17, 31, 52, 3841):
+        for lines in range(1, 8):
+            for off in (0, 1):
+                buf = torch.randint(0, 256, (ls * lines + off,), dtype=torch.uint8, device="cuda")
+                api.deinterlace(buf[off:], ls, lines)
+                n += 1
+    for ls, h in ((1, 1), (3, 7), (3841, 6)):
+        src = torch.randint(0, 256, (ls * h,), dtype=torch.uint8, device="cuda")
+        api.il_upper_to_merged(src, ls, h, dst=torch.empty_like(src))
+        api.il_merged_to_upper(src, ls, h)
+        n += 2
 torch.cuda.synchronize()
 print("exercised", n, "calls")

@@ -87,6 +87,10 @@ SIGNATURES = {
     "ugb200_yuv422pXX_to_uyvy": (_i, [_vp, _vp]),
     "ugb200_yuv422p10le_to_uyvy": (_i, [_vp, _vp]),
     "ugb200_yuv422p10le_to_v210": (_i, [_vp, _vp]),
+    "ugb200_vc_deinterlace_ex": (_i, [_i, _vp, _sz, _vp, _sz, _sz, _vp]),
+    "ugb200_vc_deinterlace": (_i, [_vp, _l, _i, _vp]),
+    "ugb200_il_upper_to_merged": (_i, [_vp, _vp, _i, _i, _vp]),
+    "ugb200_il_merged_to_upper": (_i, [_vp, _vp, _i, _i, _vp]),
     # include/ugb200_jpeg.h
     "ugb200_jpeg_default_params": (None, [_vp]),
     "ugb200_jpeg_encoder_create": (_vp, [_vp]),

@@ -149,6 +149,36 @@ def from_planar(name, planes, linesizes, width, height, out, out_pitch, in_depth
     return out
 
 
+def deinterlace_ex(codec, src, src_linesize, lines, dst=None, dst_pitch=None, stream=None):
+    """vc_deinterlace_ex (src/video_codec.c:722-854) on device tensors; dst=src for the in-place form"""
+    dst_pitch = src_linesize if dst_pitch is None else dst_pitch
+    if dst is None:
+        dst = torch.zeros(dst_pitch * lines, dtype=torch.uint8, device=src.device)
+    rc = _L.ugb200_vc_deinterlace_ex(int(codec), _ptr(src), src_linesize, _ptr(dst), dst_pitch, lines, _stream(stream))
+    _check(rc, f"ugb200_vc_deinterlace_ex({Codec(codec).name})")
+    return dst
+
+
+def deinterlace(buf, linesize, lines, stream=None):
+    """vc_deinterlace (src/video_codec.c:597-711), in place on a device tensor"""
+    _check(_L.ugb200_vc_deinterlace(_ptr(buf), linesize, lines, _stream(stream)), "ugb200_vc_deinterlace")
+    return buf
+
+
+def il_upper_to_merged(src, linesize, height, dst=None, stream=None):
+    """il_upper_to_merged (src/video_frame.c:332-355); dst=None works in place"""
+    dst = src if dst is None else dst
+    _check(_L.ugb200_il_upper_to_merged(_ptr(dst), _ptr(src), linesize, height, _stream(stream)), "ugb200_il_upper_to_merged")
+    return dst
+
+
+def il_merged_to_upper(src, linesize, height, dst=None, stream=None):
+    """il_merged_to_upper (src/video_frame.c:357-379); dst=None works in place"""
+    dst = src if dst is None else dst
+    _check(_L.ugb200_il_merged_to_upper(_ptr(dst), _ptr(src), linesize, height, _stream(stream)), "ugb200_il_merged_to_upper")
+    return dst
+
+
 class AvPlanes(ctypes.Structure):
     """struct ugb200_av_planes (include/ugb200_lavc.h): AVFrame::data / AVFrame::linesize"""
     _fields_ = [("data", ctypes.c_void_p * 4), ("linesize", ctypes.c_int * 4)]
