@@ -160,6 +160,36 @@ UGB_API int ugb200_vc_deinterlace(void *buf, long linesize, int lines, cuda_wrap
 UGB_API int ugb200_il_upper_to_merged(void *dst, void *src, int linesize, int height, cuda_wrapper_stream_t stream);
 UGB_API int ugb200_il_merged_to_upper(void *dst, void *src, int linesize, int height, cuda_wrapper_stream_t stream);
 
+/* ---- field-rate postprocessors (src/vo_postprocess/temporal-deint.c, src/vo_postprocess/interlace.c) -------- */
+/* Stateless: the caller keeps the two frame buffers, as common_getf does.  `call` 0 is the module's postprocess(in =
+ * frame) and 1 the follow-up postprocess(in = NULL); `cur` is the merged frame just received, `prev` the one before.
+ * Rows [0, height) of dst get the reference's bytes [0, linesize) and nothing else is written or read, except where
+ * noted.  Differences (DESIGN.md §8): nothing past linesize (the reference rounds 8/16-bit rows up to 16 bytes and
+ * writes 4 x linesize for R10k) nor row `height` (double_framerate at odd height) is touched; height < 2 is -1;
+ * opaque codecs are -4 for linear and :d.
+ * -1: a null pointer, height < 2, linesize == 0, pitch < linesize, call not 0 / 1, dst overlapping a source, or a
+ * 16-bit (word) codec whose addresses, linesize or pitch are not multiples of 2 (4) where the codec matters.
+ * Every refusal (-1, -4) writes nothing; -2 (a CUDA launch or scratch allocation failed) can leave dst partly written. */
+/* double_framerate (temporal-deint.c:240-277): call 0 = cur's even rows and prev's odd rows (at odd height row
+ * height-1 stays as it is), call 1 = cur.  deinterlace != 0 is `:d`: then vc_deinterlace_ex in place at pitch linesize,
+ * as ugb200_vc_deinterlace_ex computes it (-4 where that refuses); at pitch == linesize weave and blend are one pass,
+ * otherwise the first linesize * height bytes of dst are blended as the reference blends them. */
+UGB_API int ugb200_pp_double_framerate(int codec, const void *prev, const void *cur, size_t linesize, int height, int call,
+                                       int deinterlace, void *dst, size_t pitch, cuda_wrapper_stream_t stream);
+/* deinterlace_bob (:279-300): call 0 doubles rows 0, 2, ...; call 1 writes row 1 to rows 0-2, then doubles 3, 5, ...;
+ * a left-over last row repeats the row above it */
+UGB_API int ugb200_pp_bob(const void *cur, size_t linesize, int height, int call, void *dst, size_t pitch, cuda_wrapper_stream_t stream);
+/* deinterlace_linear (:442-466, avg_lines :307-440): rows of the call's parity are copied, the row between two of
+ * them is avg_lines of the two, the last row(s) repeat the last copied row.  avg_lines as the reference computes
+ * it: 8/16-bit c1/2 + c2/2 + (c1 & 1), v210 whole 16-byte groups, R10k byte-swapped with bits 0-1 zero, R12L
+ * over linesize/16 groups of 4 words with the last word dropped unless 3 divides linesize/16; DVS10 copies */
+UGB_API int ugb200_pp_linear(int codec, const void *cur, size_t linesize, int height, int call, void *dst, size_t pitch,
+                             cuda_wrapper_stream_t stream);
+/* interlace (interlace.c:159-190): out row i = row i of even_rows (the module's s->odd) for even i, of odd_rows
+ * (s->even) for odd i */
+UGB_API int ugb200_pp_interlace(const void *even_rows, const void *odd_rows, size_t linesize, int height, void *dst, size_t pitch,
+                                cuda_wrapper_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

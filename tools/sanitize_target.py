@@ -260,5 +260,23 @@ if ONLY not in ("jpeg", "staged"):
         api.il_upper_to_merged(src, ls, h, dst=torch.empty_like(src))
         api.il_merged_to_upper(src, ls, h)
         n += 2
+    # field-rate postprocessors on tight buffers (sources L * h, dst ends at row h-1's L bytes): R10k and R12L at line sizes
+    # off 16 and 36, an odd 8-bit line size, odd h and h = 2, both calls, `:d` fused (pitch L) and composed (pitch > L)
+    for codec, ls in ((5, 68), (5, 7680 * 4), (6, 36 * 5 + 8), (6, 36 * 3 + 4), (2, 47), (7, 1004 // 4 * 4), (27, 11508)):
+        for h in (2, 3, 5, 7):
+            for pitch in (ls, ls + 12):
+                prev = torch.randint(0, 256, (ls * h,), dtype=torch.uint8, device="cuda")
+                cur = torch.randint(0, 256, (ls * h,), dtype=torch.uint8, device="cuda")
+                dst = torch.zeros(pitch * (h - 1) + ls, dtype=torch.uint8, device="cuda")
+                for call in (0, 1):
+                    api.deinterlace_bob(cur, ls, h, call, dst=dst, pitch=pitch)
+                    api.deinterlace_linear(codec, cur, ls, h, call, dst=dst, pitch=pitch)
+                    api.double_framerate(codec, prev, cur, ls, h, call, dst=dst, pitch=pitch)
+                    if pitch == ls or pitch % 4 == 0:
+                        api.double_framerate(codec, prev, cur, ls, h, call, True, dst=dst, pitch=pitch)
+                        n += 1
+                    n += 3
+                api.interlace(cur, prev, ls, h, dst=dst, pitch=pitch)
+                n += 1
 torch.cuda.synchronize()
 print("exercised", n, "calls")

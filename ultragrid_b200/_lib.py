@@ -91,6 +91,10 @@ SIGNATURES = {
     "ugb200_vc_deinterlace": (_i, [_vp, _l, _i, _vp]),
     "ugb200_il_upper_to_merged": (_i, [_vp, _vp, _i, _i, _vp]),
     "ugb200_il_merged_to_upper": (_i, [_vp, _vp, _i, _i, _vp]),
+    "ugb200_pp_double_framerate": (_i, [_i, _vp, _vp, _sz, _i, _i, _i, _vp, _sz, _vp]),
+    "ugb200_pp_bob": (_i, [_vp, _sz, _i, _i, _vp, _sz, _vp]),
+    "ugb200_pp_linear": (_i, [_i, _vp, _sz, _i, _i, _vp, _sz, _vp]),
+    "ugb200_pp_interlace": (_i, [_vp, _vp, _sz, _i, _vp, _sz, _vp]),
     # include/ugb200_jpeg.h
     "ugb200_jpeg_default_params": (None, [_vp]),
     "ugb200_jpeg_encoder_create": (_vp, [_vp]),

@@ -179,6 +179,48 @@ def il_merged_to_upper(src, linesize, height, dst=None, stream=None):
     return dst
 
 
+def _pp_out(src, linesize, height, dst, pitch):
+    """dst=None allocates a zeroed frame: double_framerate's call 0 at odd height leaves row height-1 as it finds it
+    (and `:d` blends it into row height-2), as the reference does"""
+    pitch = linesize if pitch is None else pitch
+    if dst is None:
+        dst = torch.zeros(pitch * height, dtype=torch.uint8, device=src.device)
+    return dst, pitch
+
+
+def double_framerate(codec, prev, cur, linesize, height, call, deinterlace=False, dst=None, pitch=None, stream=None):
+    """double_framerate (src/vo_postprocess/temporal-deint.c:240-277) on device tensors: call 0 weaves cur's even rows
+    with prev's odd rows, call 1 is cur; deinterlace=True is the `:d` option.  At odd height call 0 leaves row height-1 of
+    dst as it is, and `:d` blends it into row height-2, as the reference does: pass dst=None for a zeroed frame."""
+    dst, pitch = _pp_out(cur, linesize, height, dst, pitch)
+    rc = _L.ugb200_pp_double_framerate(int(codec), _ptr(prev), _ptr(cur), linesize, height, call, int(bool(deinterlace)), _ptr(dst), pitch,
+                                       _stream(stream))
+    _check(rc, f"ugb200_pp_double_framerate({Codec(codec).name})")
+    return dst
+
+
+def deinterlace_bob(cur, linesize, height, call, dst=None, pitch=None, stream=None):
+    """deinterlace_bob (src/vo_postprocess/temporal-deint.c:279-300): call 0 doubles the even rows, call 1 the odd"""
+    dst, pitch = _pp_out(cur, linesize, height, dst, pitch)
+    _check(_L.ugb200_pp_bob(_ptr(cur), linesize, height, call, _ptr(dst), pitch, _stream(stream)), "ugb200_pp_bob")
+    return dst
+
+
+def deinterlace_linear(codec, cur, linesize, height, call, dst=None, pitch=None, stream=None):
+    """deinterlace_linear (src/vo_postprocess/temporal-deint.c:442-466): the call's field, missing rows interpolated"""
+    dst, pitch = _pp_out(cur, linesize, height, dst, pitch)
+    rc = _L.ugb200_pp_linear(int(codec), _ptr(cur), linesize, height, call, _ptr(dst), pitch, _stream(stream))
+    _check(rc, f"ugb200_pp_linear({Codec(codec).name})")
+    return dst
+
+
+def interlace(even_rows, odd_rows, linesize, height, dst=None, pitch=None, stream=None):
+    """interlace (src/vo_postprocess/interlace.c:159-190): out row i from even_rows for even i, from odd_rows for odd i"""
+    dst, pitch = _pp_out(even_rows, linesize, height, dst, pitch)
+    _check(_L.ugb200_pp_interlace(_ptr(even_rows), _ptr(odd_rows), linesize, height, _ptr(dst), pitch, _stream(stream)), "ugb200_pp_interlace")
+    return dst
+
+
 class AvPlanes(ctypes.Structure):
     """struct ugb200_av_planes (include/ugb200_lavc.h): AVFrame::data / AVFrame::linesize"""
     _fields_ = [("data", ctypes.c_void_p * 4), ("linesize", ctypes.c_int * 4)]
