@@ -190,6 +190,45 @@ UGB_API int ugb200_pp_linear(int codec, const void *cur, size_t linesize, int he
 UGB_API int ugb200_pp_interlace(const void *even_rows, const void *odd_rows, size_t linesize, int height, void *dst, size_t pitch,
                                 cuda_wrapper_stream_t stream);
 
+/* ---- colour capture filters (src/capture_filter/gamma.cpp, matrix.c, matrix2.c, grayscale.c) -------------------- */
+/* The filters' filter() on device frames; each is also a postprocessor through ADD_VO_PP_CAPTURE_FILTER_WRAPPER.
+ * Frames are tight (vc_get_linesize pitch, which the vo_pp wrapper insists on); input and output lengths follow
+ * from codec, width and height as vf_alloc_desc derives them.  Every double -> integer conversion is x86's
+ * cvttsd2si with a 32-bit destination (truncation, INT_MIN for NaN and out-of-range values), then the low 8 or 16
+ * bits; FP64 sums run left to right without FMA.  Differences (DESIGN.md §8): gamma maps every sample (the
+ * reference skips the last len % hardware_concurrency() ones); nothing is written past the output frame (matrix
+ * UYVY at odd widths stops at 3 * w * h, matrix2 v210 at the frame's length); matrix2 on v210 maps every 16-byte
+ * group of the frame, including those >= w * h / 6 whose reference bytes are indeterminate.
+ * -1: a null pointer or handle, width or height <= 0, out_depth not 0 / 8 / 16, dst overlapping src, or a 16-bit
+ * buffer at an odd address (v210: not a multiple of 4).  -4: a codec the filter does not take (the reference
+ * returns NULL for gamma and matrix, its input for grayscale, and a frame of uninitialised memory for matrix2).
+ * Every refusal (-1, -4) writes nothing; -2 is a failed launch. */
+
+/* gamma:g[:8|:16] (gamma.cpp): the four tables pow(i / max_in, g) * max_out (8->8, 16->16, 8->16, 16->8), built
+ * on the host with the C library's pow at create; NULL when the device allocation fails */
+typedef struct ugb200_cf_gamma *ugb200_cf_gamma_t;
+UGB_API ugb200_cf_gamma_t ugb200_cf_gamma_create(double gamma);
+UGB_API void ugb200_cf_gamma_destroy(ugb200_cf_gamma_t g);
+/* codec RGB or RG48; out_depth 0 keeps the depth, 8 writes RGB, 16 RG48 */
+UGB_API int ugb200_cf_gamma(ugb200_cf_gamma_t g, int codec, int out_depth, int width, int height, const void *src, void *dst,
+                            cuda_wrapper_stream_t stream);
+/* matrix:a:...:i[:no-bound-check] (matrix.c): UYVY -> RGB (U Y0 V Y1 -> (Y0-16, U-128, V-128), (Y1-16, ...)),
+ * RGB -> RGB, RG48 -> RG48; out = (m0*a0 + m1*a1) + m2*a2 per row.  check_bounds != 0 clamps the int32 to
+ * [0, 255], RG48 included; 0 keeps its low bits.  UYVY at odd widths drifts across rows as the reference does. */
+UGB_API int ugb200_cf_matrix(int codec, int width, int height, const double m[9], int check_bounds, const void *src, void *dst,
+                             cuda_wrapper_stream_t stream);
+/* matrix2:a:...:i or matrix2:y601_to_y709 (matrix2.c): YCbCr in place of its own codec, no clamping.
+ * UYVY: Y' = ((16 + m0*y) + m1*u) + m2*v, U' / V' the same with offset 128 and y = (y1 + y2) / 2.
+ * Y416: offsets 1<<12 / 1<<15 per pixel, A = 0xFFFF.  v210: the 16-byte group x of the frame -> 6 Y416 pixels
+ * (vc_copylineV210toY416) -> the Y416 matrix -> vc_copylineY416toV210 (pair-averaged chroma, >> 6) -> group x. */
+UGB_API int ugb200_cf_matrix2(int codec, int width, int height, const double m[9], const void *src, void *dst,
+                              cuda_wrapper_stream_t stream);
+/* matrix2.c's y601_y709_matrix, the coefficients of `matrix2:y601_to_y709` */
+#define UGB200_CF_Y601_TO_Y709 { 1, -0.11555, -0.207938, 0, 1.01864, 0.114618, 0, 0.075049, 1.025327 }
+/* grayscale (grayscale.c): UYVY, chroma bytes 127 and luma copied over the first 2 * w * h bytes; at odd widths
+ * the last 2 * h bytes of the frame are left as they are, as the reference leaves them */
+UGB_API int ugb200_cf_grayscale(int width, int height, const void *src, void *dst, cuda_wrapper_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

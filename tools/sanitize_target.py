@@ -278,5 +278,27 @@ if ONLY not in ("jpeg", "staged"):
                     n += 3
                 api.interlace(cur, prev, ls, h, dst=dst, pitch=pitch)
                 n += 1
+    # colour capture filters on tight buffers (input and output frames exactly vf_alloc_desc's length) at odd sizes:
+    # matrix UYVY at odd widths (the output stops at 3 * w * h), v210 off multiples of 48, RG48 / Y416 at 2-byte offsets
+    cf_g = api.gamma(2.2)
+    for w, h in ((1, 1), (3, 5), (47, 3), (49, 7), (131, 2), (1919, 3)):
+        m = api.Y601_TO_Y709
+        for c in (2, 12, 27):
+            src = torch.randint(0, 256, (vc_get_linesize(w, c) * h,), dtype=torch.uint8, device="cuda")
+            for b in (True, False):
+                api.matrix(c, src, w, h, m, b)
+                n += 1
+        for c in (2, 7, 31):
+            src = torch.randint(0, 256, (vc_get_linesize(w, c) * h,), dtype=torch.uint8, device="cuda")
+            api.matrix2(c, src, w, h, m)
+            n += 1
+        api.grayscale(torch.randint(0, 256, (vc_get_linesize(w, 2) * h,), dtype=torch.uint8, device="cuda"), w, h)
+        n += 1
+        for c in (12, 27):
+            raw = torch.randint(0, 256, (vc_get_linesize(w, c) * h + 2,), dtype=torch.uint8, device="cuda")
+            for d in (0, 8, 16):
+                cf_g(c, raw[2:], w, h, d)
+                n += 1
+    cf_g.close()
 torch.cuda.synchronize()
 print("exercised", n, "calls")

@@ -95,6 +95,12 @@ SIGNATURES = {
     "ugb200_pp_bob": (_i, [_vp, _sz, _i, _i, _vp, _sz, _vp]),
     "ugb200_pp_linear": (_i, [_i, _vp, _sz, _i, _i, _vp, _sz, _vp]),
     "ugb200_pp_interlace": (_i, [_vp, _vp, _sz, _i, _vp, _sz, _vp]),
+    "ugb200_cf_gamma_create": (_vp, [ctypes.c_double]),
+    "ugb200_cf_gamma_destroy": (None, [_vp]),
+    "ugb200_cf_gamma": (_i, [_vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "ugb200_cf_matrix": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _vp]),
+    "ugb200_cf_matrix2": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp]),
+    "ugb200_cf_grayscale": (_i, [_i, _i, _vp, _vp, _vp]),
     # include/ugb200_jpeg.h
     "ugb200_jpeg_default_params": (None, [_vp]),
     "ugb200_jpeg_encoder_create": (_vp, [_vp]),

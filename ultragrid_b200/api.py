@@ -221,6 +221,72 @@ def interlace(even_rows, odd_rows, linesize, height, dst=None, pitch=None, strea
     return dst
 
 
+# matrix2.c's y601_y709_matrix (`matrix2:y601_to_y709`), as UGB200_CF_Y601_TO_Y709 in include/ugb200.h
+Y601_TO_Y709 = (1, -0.11555, -0.207938, 0, 1.01864, 0.114618, 0, 0.075049, 1.025327)
+
+
+def _cf_out(src, nbytes, dst):
+    """dst=None allocates a zeroed frame: grayscale leaves the last 2 * h bytes of an odd-width frame as it finds them"""
+    return torch.zeros(nbytes, dtype=torch.uint8, device=src.device) if dst is None else dst
+
+
+def _matrix9(m):
+    m = (ctypes.c_double * 9)(*[float(x) for x in m])
+    assert len(m) == 9
+    return m
+
+
+class gamma:
+    """gamma:g[:8|:16] (src/capture_filter/gamma.cpp): holds the four tables, built once on the host, on the device"""
+
+    def __init__(self, g):
+        self.g = float(g)
+        self._h = _L.ugb200_cf_gamma_create(self.g)
+        if not self._h:
+            raise RuntimeError("ugb200_cf_gamma_create failed")
+
+    def __call__(self, codec, src, width, height, out_depth=0, dst=None, stream=None):
+        """RGB or RG48 in; out_depth 0 keeps the depth, 8 gives RGB, 16 RG48"""
+        in_bits = 8 if Codec(codec) == Codec.RGB else 16
+        out_bits = out_depth or in_bits
+        dst = _cf_out(src, width * height * 3 * out_bits // 8, dst)
+        rc = _L.ugb200_cf_gamma(self._h, int(codec), int(out_depth), width, height, _ptr(src), _ptr(dst), _stream(stream))
+        _check(rc, f"ugb200_cf_gamma({Codec(codec).name}, {out_depth})")
+        return dst
+
+    def close(self):
+        if self._h:
+            _L.ugb200_cf_gamma_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+
+def matrix(codec, src, width, height, m, check_bounds=True, dst=None, stream=None):
+    """matrix:a:...:i[:no-bound-check] (src/capture_filter/matrix.c): UYVY -> RGB, RGB -> RGB, RG48 -> RG48"""
+    out_codec = Codec.RGB if Codec(codec) == Codec.UYVY else codec
+    dst = _cf_out(src, vc_get_linesize(width, out_codec) * height, dst)
+    rc = _L.ugb200_cf_matrix(int(codec), width, height, _matrix9(m), int(bool(check_bounds)), _ptr(src), _ptr(dst), _stream(stream))
+    _check(rc, f"ugb200_cf_matrix({Codec(codec).name})")
+    return dst
+
+
+def matrix2(codec, src, width, height, m=Y601_TO_Y709, dst=None, stream=None):
+    """matrix2:a:...:i (src/capture_filter/matrix2.c) on UYVY, v210 or Y416, in the same codec"""
+    dst = _cf_out(src, vc_get_linesize(width, codec) * height, dst)
+    rc = _L.ugb200_cf_matrix2(int(codec), width, height, _matrix9(m), _ptr(src), _ptr(dst), _stream(stream))
+    _check(rc, f"ugb200_cf_matrix2({Codec(codec).name})")
+    return dst
+
+
+def grayscale(src, width, height, dst=None, stream=None):
+    """grayscale (src/capture_filter/grayscale.c) on UYVY: chroma 127, luma copied over the first 2 * w * h bytes"""
+    dst = _cf_out(src, vc_get_linesize(width, Codec.UYVY) * height, dst)
+    _check(_L.ugb200_cf_grayscale(width, height, _ptr(src), _ptr(dst), _stream(stream)), "ugb200_cf_grayscale")
+    return dst
+
+
 class AvPlanes(ctypes.Structure):
     """struct ugb200_av_planes (include/ugb200_lavc.h): AVFrame::data / AVFrame::linesize"""
     _fields_ = [("data", ctypes.c_void_p * 4), ("linesize", ctypes.c_int * 4)]
