@@ -229,6 +229,59 @@ UGB_API int ugb200_cf_matrix2(int codec, int width, int height, const double m[9
  * the last 2 * h bytes of the frame are left as they are, as the reference leaves them */
 UGB_API int ugb200_cf_grayscale(int width, int height, const void *src, void *dst, cuda_wrapper_stream_t stream);
 
+/* ---- geometry filters (src/capture_filter/flip.c, mirror.c, src/vo_postprocess/crop.c, src/utils/vf_split.cpp,
+ * src/vo_postprocess/border.c, 3d-interlaced.c) -------------------------------------------------------------------
+ * The filters that move bytes without changing them (interlaced_3d averages two rows).  Stateless: the caller keeps
+ * the module's options.  Frames are tight (vc_get_linesize pitch) unless a pitch is taken.  Every byte the reference
+ * writes inside the output frame from bytes inside the sources gets the reference's value.  Differences (DESIGN.md
+ * §8): nothing is written past the output frame, into the tails of split's tile rows or into pitch padding the
+ * reference leaves alone; bytes the reference computes from memory past a source are left unwritten.
+ * -1: a null pointer, width or height <= 0, dst overlapping a source, or the arguments under which the reference
+ * asserts, crashes or writes outside the frame (noted per function).  -4: a codec the filter does not take.
+ * Every refusal (-1, -4) writes nothing; -2 is a failed launch or scratch allocation. */
+/* flip (flip.c:65-80): out row h-1-y = in row y, vc_get_linesize(width) bytes; any codec with a byte layout */
+UGB_API int ugb200_cf_flip(int codec, int width, int height, const void *src, void *dst, cuda_wrapper_stream_t stream);
+/* mirror (mirror.c:50-95): UYVY only (-4 otherwise, where the reference returns its input): group k of a row,
+ * (U Y0 V Y1), lands at byte L - 4 - 4k as (U Y1 V Y0) */
+UGB_API int ugb200_cf_mirror(int codec, int width, int height, const void *src, void *dst, cuda_wrapper_stream_t stream);
+/* crop:[size=WxH][:width=W][:height=H][:xoff=X][:yoff=Y] (crop.c): out = {output width, output height, xoff, yoff}
+ * exactly as crop_postprocess_reconfigure (:118-136) and crop_postprocess (:165-172) compute them: the width rounded
+ * to whole pixel blocks in double arithmetic, the offsets compared in unsigned arithmetic (a negative offset is
+ * clamped to in - out only when the sum wraps).  width / height 0 keep the input's.  -4: a codec without a pixel
+ * block (opaque, planar or DXT). */
+UGB_API int ugb200_cf_crop_geometry(int codec, int in_width, int in_height, int width, int height, int xoff, int yoff, int out[4]);
+/* crop_postprocess (:160-185): out row y, at y * pitch, gets `pitch` bytes from source byte (yoff + y) * src_linesize
+ * + xoff_bytes (xoff_bytes = xoff * bpp rounded down to whole blocks), reading on into the rest of the source row and
+ * the next; bytes past the source frame are left unwritten.  pitch 0 is the capture filter's
+ * vc_get_linesize(output width) (cf_crop_filter :214); the postprocessor passes the display's pitch.
+ * An empty output frame (a window narrower than one pixel block) writes nothing and returns 0; dst may then be NULL.
+ * -1 also: an unclamped negative offset that makes the first row start before the source. */
+UGB_API int ugb200_cf_crop(int codec, int in_width, int in_height, int width, int height, int xoff, int yoff, const void *src,
+                           void *dst, size_t pitch, cuda_wrapper_stream_t stream);
+/* split:X:Y (split.c, vo_postprocess/split.c, vf_split.cpp:14-84): tiles[(line / tile_h) * x + i] row line % tile_h, at
+ * vc_get_linesize(tile_w) pitch, gets (size_t) (tile_w * bpp) bytes from source row `line` at byte offset
+ * `unsigned byte += tile_w * bpp` (truncated at every step); the rest of each tile row is left unwritten.  All
+ * x * y tiles in one launch; the tile table goes to stream-ordered scratch.  -1 also: width % x or height % y != 0
+ * (the reference asserts).  -4: a codec without a pixel block. */
+UGB_API int ugb200_cf_split(int codec, int width, int height, int x, int y, const void *src, void *const *tiles,
+                            cuda_wrapper_stream_t stream);
+/* border[:color=rrggbb][:width=W][:height=H] (border.c:104-190): color = the module state's four RGBA bytes (as
+ * border_init parses them), border_width / border_height as the state holds them.  Rows [bh, h - bh) are copied
+ * outside the side bands, every other byte is the fill, each byte written once.  UYVY: the 4 bytes
+ * vc_copylineRGBAtoUYVY makes from two pixels of the colour, over whole rows and over bytes [0, 4g) and [L - 4g, L)
+ * of every row, g = (border_width + 1) / 2.  RGB / RGBA: color[b % bpp] over whole rows and border_width pixels on
+ * each side.  -4: other codecs (the reference copies the middle rows, then fails).  -1 also: 2 * border_height >
+ * height, or a side band wider than the row. */
+UGB_API int ugb200_pp_border(int codec, int width, int height, const unsigned char color[4], unsigned border_width, unsigned border_height,
+                             const void *src, void *dst, cuda_wrapper_stream_t stream);
+/* interlaced_3d (3d-interlaced.c:131-167): left and right eye tiles -> one frame; out row x is written from byte
+ * x * Lc, Lc = L rounded up to 16, in 16-byte chunks, chunk c = pavgb ((a + b + 1) >> 1) of bytes [16c, 16c + 16) of
+ * rows x/2*2 and x/2*2+1 of tile x % 2 (L = vc_get_linesize(width)).  Rows drift when L % 16 != 0, as the
+ * reference's do.  Bytes at or past L * height, and bytes whose sources lie past a tile (the last row at odd height
+ * reads row `height` of the left tile), are not written. */
+UGB_API int ugb200_pp_interlaced_3d(int codec, int width, int height, const void *left, const void *right, void *dst,
+                                    cuda_wrapper_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

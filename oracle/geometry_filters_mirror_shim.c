@@ -1,0 +1,29 @@
+// TEST INFRASTRUCTURE: the UNMODIFIED src/capture_filter/mirror.c, included where it lies under $(REF), with its
+// static functions exposed to tests/test_geometry_filters.py.
+#include "capture_filter/mirror.c"
+
+/// filter() with the output through the vo_pp_out_buffer hook: 0, or 1 where filter returns its input (not UYVY)
+int ref_mirror_filter(int codec, int width, int height, char *in, char *out)
+{
+        void *st = NULL;
+        if (init(NULL, "", &st) != 0) {
+                return -2;
+        }
+        vo_pp_set_out_buffer(st, out);
+        struct video_frame *f = vf_alloc(1);
+        f->color_spec = (codec_t) codec;
+        f->interlacing = PROGRESSIVE;
+        f->fps = 30;
+        f->tiles[0].width = width;
+        f->tiles[0].height = height;
+        f->tiles[0].data = in;
+        f->tiles[0].data_len = vc_get_linesize(width, (codec_t) codec) * height;
+        struct video_frame *o = filter(st, f);
+        const int rc = o == f ? 1 : 0;
+        if (o != f) {
+                VIDEO_FRAME_DISPOSE(o);
+        }
+        vf_free(f);
+        done(st);
+        return rc;
+}

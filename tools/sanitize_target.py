@@ -300,5 +300,28 @@ if ONLY not in ("jpeg", "staged"):
                 cf_g(c, raw[2:], w, h, d)
                 n += 1
     cf_g.close()
+    # geometry filters on tight buffers (each allocation exactly the frame, so a read or write past it is out of
+    # bounds) at odd line sizes and misaligned offsets: RGB crops at 3-byte offsets, v210 split columns, the largest
+    # tile count (one tile per pixel column and row), interlaced_3d with drifted rows
+    def tight(nbytes, off=0):
+        return torch.randint(0, 256, (nbytes + off,), dtype=torch.uint8, device="cuda")[off:]
+    for w, h in ((1, 1), (3, 5), (47, 3), (131, 7), (1919, 3)):
+        for c in (2, 7, 12):
+            for off in (0, 1, 3, 15):
+                src = tight(vc_get_linesize(w, c) * h, off)
+                api.flip(c, src, w, h, dst=tight(src.numel(), (off * 5) % 16))
+                api.interlaced_3d(c, src, tight(src.numel(), 3), w, h, dst=tight(src.numel(), off))
+                api.crop(c, src, w, h, max(w // 2, 1), max(h // 2, 1), w // 3 + 1, h // 3)
+                api.crop(c, src, w, h, max(w // 2, 1), max(h // 2, 1), w // 3 + 1, h // 3, pitch=vc_get_linesize(w, c) + 3)
+                n += 4
+                if c != 7:
+                    api.border(c, src, w, h, (1, 2, 3, 4), min(w, 2) if c != 2 else min(2 * ((w + 1) // 2), 2), h // 2 // 2 * 2)
+                    n += 1
+                if c == 2:
+                    api.mirror(c, src, w, h, dst=tight(src.numel(), off))
+                    n += 1
+        for c, x, y in ((7, 1, 1), (12, w, h), (2, 1, h), (7, w, 1)):
+            api.split(c, tight(vc_get_linesize(w, c) * h, 1), w, h, x, y)
+            n += 1
 torch.cuda.synchronize()
 print("exercised", n, "calls")

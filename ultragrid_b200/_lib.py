@@ -101,6 +101,13 @@ SIGNATURES = {
     "ugb200_cf_matrix": (_i, [_i, _i, _i, _vp, _i, _vp, _vp, _vp]),
     "ugb200_cf_matrix2": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp]),
     "ugb200_cf_grayscale": (_i, [_i, _i, _vp, _vp, _vp]),
+    "ugb200_cf_flip": (_i, [_i, _i, _i, _vp, _vp, _vp]),
+    "ugb200_cf_mirror": (_i, [_i, _i, _i, _vp, _vp, _vp]),
+    "ugb200_cf_crop_geometry": (_i, [_i, _i, _i, _i, _i, _i, _i, ctypes.POINTER(_i)]),
+    "ugb200_cf_crop": (_i, [_i, _i, _i, _i, _i, _i, _i, _vp, _vp, _sz, _vp]),
+    "ugb200_cf_split": (_i, [_i, _i, _i, _i, _i, _vp, ctypes.POINTER(_vp), _vp]),
+    "ugb200_pp_border": (_i, [_i, _i, _i, ctypes.POINTER(ctypes.c_uint8), ctypes.c_uint, ctypes.c_uint, _vp, _vp, _vp]),
+    "ugb200_pp_interlaced_3d": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp]),
     # include/ugb200_jpeg.h
     "ugb200_jpeg_default_params": (None, [_vp]),
     "ugb200_jpeg_encoder_create": (_vp, [_vp]),

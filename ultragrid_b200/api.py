@@ -287,6 +287,63 @@ def grayscale(src, width, height, dst=None, stream=None):
     return dst
 
 
+def flip(codec, src, width, height, dst=None, stream=None):
+    """flip (src/capture_filter/flip.c): out row h-1-y = in row y"""
+    dst = _cf_out(src, vc_get_linesize(width, codec) * height, dst)
+    _check(_L.ugb200_cf_flip(int(codec), width, height, _ptr(src), _ptr(dst), _stream(stream)), "ugb200_cf_flip")
+    return dst
+
+
+def mirror(codec, src, width, height, dst=None, stream=None):
+    """mirror (src/capture_filter/mirror.c): UYVY rows reversed group by group, the two lumas of each group swapped"""
+    dst = _cf_out(src, vc_get_linesize(width, Codec.UYVY) * height, dst)
+    _check(_L.ugb200_cf_mirror(int(codec), width, height, _ptr(src), _ptr(dst), _stream(stream)), "ugb200_cf_mirror")
+    return dst
+
+
+def crop_geometry(codec, in_width, in_height, width=0, height=0, xoff=0, yoff=0):
+    """(output width, output height, xoff, yoff) as crop.c computes them for crop:size=WxH:xoff=X:yoff=Y"""
+    out = (ctypes.c_int * 4)()
+    _check(_L.ugb200_cf_crop_geometry(int(codec), in_width, in_height, width, height, xoff, yoff, out), "ugb200_cf_crop_geometry")
+    return tuple(out)
+
+
+def crop(codec, src, in_width, in_height, width=0, height=0, xoff=0, yoff=0, pitch=0, dst=None, stream=None):
+    """crop (src/vo_postprocess/crop.c): pitch 0 is the capture filter's vc_get_linesize(output width)"""
+    ow, oh, _, _ = crop_geometry(codec, in_width, in_height, width, height, xoff, yoff)
+    pitch = pitch or vc_get_linesize(ow, codec)
+    dst = _cf_out(src, pitch * oh, dst)
+    rc = _L.ugb200_cf_crop(int(codec), in_width, in_height, width, height, xoff, yoff, _ptr(src), _ptr(dst), pitch, _stream(stream))
+    _check(rc, "ugb200_cf_crop")
+    return dst
+
+
+def split(codec, src, width, height, x, y, tiles=None, stream=None):
+    """split:X:Y (src/utils/vf_split.cpp): a list of x * y tile tensors of vc_get_linesize(width / x) * (height / y) bytes"""
+    if tiles is None:
+        n = vc_get_linesize(width // x, codec) * (height // y) if x > 0 and y > 0 else 0
+        tiles = [torch.zeros(n, dtype=torch.uint8, device=src.device) for _ in range(max(x * y, 0))]
+    ptrs = (ctypes.c_void_p * max(len(tiles), 1))(*[t.data_ptr() for t in tiles])
+    _check(_L.ugb200_cf_split(int(codec), width, height, x, y, _ptr(src), ptrs, _stream(stream)), "ugb200_cf_split")
+    return tiles
+
+
+def border(codec, src, width, height, color=(0xff, 0xff, 0x00, 0xff), border_width=10, border_height=10, dst=None, stream=None):
+    """border (src/vo_postprocess/border.c): color = the module state's four RGBA bytes; the defaults are border_init's"""
+    dst = _cf_out(src, vc_get_linesize(width, codec) * height, dst)
+    col = (ctypes.c_uint8 * 4)(*color)
+    rc = _L.ugb200_pp_border(int(codec), width, height, col, border_width, border_height, _ptr(src), _ptr(dst), _stream(stream))
+    _check(rc, "ugb200_pp_border")
+    return dst
+
+
+def interlaced_3d(codec, left, right, width, height, dst=None, stream=None):
+    """interlaced_3d (src/vo_postprocess/3d-interlaced.c): two eye tiles -> one line-interleaved, pair-averaged frame"""
+    dst = _cf_out(left, vc_get_linesize(width, codec) * height, dst)
+    rc = _L.ugb200_pp_interlaced_3d(int(codec), width, height, _ptr(left), _ptr(right), _ptr(dst), _stream(stream))
+    _check(rc, "ugb200_pp_interlaced_3d")
+    return dst
+
 class AvPlanes(ctypes.Structure):
     """struct ugb200_av_planes (include/ugb200_lavc.h): AVFrame::data / AVFrame::linesize"""
     _fields_ = [("data", ctypes.c_void_p * 4), ("linesize", ctypes.c_int * 4)]
