@@ -282,6 +282,43 @@ UGB_API int ugb200_pp_border(int codec, int width, int height, const unsigned ch
 UGB_API int ugb200_pp_interlaced_3d(int codec, int width, int height, const void *left, const void *right, void *dst,
                                     cuda_wrapper_stream_t stream);
 
+/* ---- logo and the R12L <-> Y416 pass-through filters (src/capture_filter/logo.c, r12l_to_y416_fake.c,
+ * src/vo_postprocess/y416_to_r12l_fake.c) ----------------------------------------------------------------------------
+ * Frames are tight (vc_get_linesize pitch) unless a pitch is taken.  Differences (DESIGN.md §8): logo widths whose
+ * RGB segment the reference allocates too short are blended as the reference blends them with a long enough
+ * segment; where the reference writes past a row or the frame, or asserts, the call returns -1.
+ * -1: a null pointer or handle, a size <= 0, and the cases noted per function.  -4: a codec the filter does not
+ * take.  Every refusal (-1, -4) writes nothing; -2 is a failed launch. */
+/* logo:<file>[:<x>[:<y>]] (logo.c:162-235): the module state's logo, s->logo (RGBA; load_logo_data_from_file widens
+ * 3-channel PAMs to alpha 0xFF), copied to the device; NULL when a size is 0 or the device allocation fails */
+typedef struct ugb200_cf_logo *ugb200_cf_logo_t;
+UGB_API ugb200_cf_logo_t ugb200_cf_logo_create(const unsigned char *rgba, unsigned width, unsigned height);
+UGB_API void ugb200_cf_logo_destroy(ugb200_cf_logo_t logo);
+/* filter() in place on a w x h logo over a width x height frame of RGB, RGBA, UYVY, RG48 or R12L (-4 otherwise, where
+ * the reference returns its input).  x, y: the state's ints, -1 the default (bottom right).  rect_x = x, or width - w
+ * when x < 0 or x + w > width, then C-truncated to a multiple of get_pf_block_bytes (bytes, counted in pixels);
+ * rect_y = y, or height - h.  A negative rect_x or rect_y returns 0 and writes nothing.  Rows [rect_y, rect_y + h)
+ * get bytes [off, off + vc_get_linesize(w)), off = vc_get_linesize(rect_x), and nothing else: the span is decoded
+ * to RGB (the decoder_t of get_decoder_from_to(codec, RGB), default shifts), its first w pixels blended with the
+ * logo as (p * (255 - a) + l * a) / 255 in int, and the span encoded back (get_decoder_from_to(RGB, codec)).  Every
+ * pixel of the span makes the round trip: UYVY through A4 then A5, RG48 with its low bytes zeroed, RGBA with alpha
+ * 0xFF and the decoder's SSSE3 tail (pixels [d - 4, d) of the row, d = w rounded up to 4, all take pixel d - 4's
+ * colour before the blend), R12L through 8 bits.  -1 also: off + vc_get_linesize(w) > vc_get_linesize(width) (the
+ * reference writes into the next row or past the frame), RG48 / R12L frames at an address not a multiple of 2 / 4. */
+UGB_API int ugb200_cf_logo(ugb200_cf_logo_t logo, int codec, int width, int height, int x, int y, void *frame,
+                           cuda_wrapper_stream_t stream);
+/* r12l_to_y416_fake[:full-range] (r12l_to_y416_fake.c:85-191): tight R12L -> tight Y416, each pixel (R', G', B',
+ * 0xFFFF) as uint16: full range c << 4; limited 14 * R + 4096, 13 * G + 4096, 14 * B + 4096.
+ * -1 also: width % 8 != 0 (the reference asserts), src not 4-byte aligned, dst at an odd address, dst overlapping src. */
+UGB_API int ugb200_cf_r12l_to_y416_fake(int width, int height, int full_range, const void *src, void *dst, cuda_wrapper_stream_t stream);
+/* y416_to_r12l_fake[:full-range] (y416_to_r12l_fake.c:117-238): tight Y416 -> R12L rows at `pitch`, row y at
+ * y * pitch (the reference's single-task layout, DESIGN.md §8), alpha dropped: full range min(v >> 4, 4095);
+ * limited min((max(v, 4096) - 4096) / 14, 4095) for R and B, / 13 for G.  Pitch padding is not written.
+ * -1 also: width % 8 != 0, pitch < vc_get_linesize(width, R12L), src at an odd address, dst not 4-byte aligned,
+ * dst overlapping src. */
+UGB_API int ugb200_pp_y416_to_r12l_fake(int width, int height, int full_range, const void *src, void *dst, size_t pitch,
+                                        cuda_wrapper_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -323,5 +323,24 @@ if ONLY not in ("jpeg", "staged"):
         for c, x, y in ((7, 1, 1), (12, w, h), (2, 1, h), (7, w, 1)):
             api.split(c, tight(vc_get_linesize(w, c) * h, 1), w, h, x, y)
             n += 1
+    # logo and the R12L <-> Y416 pair on tight buffers: odd logo widths (the short-segment ones included), R12L at
+    # rect_x offsets inside a block, the span ending at the row's end and the rectangle on the frame's last row
+    for c in (12, 1, 2, 27, 6):
+        for W, H, lw, lh, x, y in ((1, 1, 1, 1, -1, -1), (47, 3, 13, 2, -1, -1), (131, 7, 37, 7, 5, 0), (131, 7, 131, 7, -1, -1),
+                                   (216, 3, 71, 3, -1, -1), (216, 3, 41, 2, 100, -1), (1919, 3, 150, 3, -1, -1)):
+            lg = api.logo(torch.randint(0, 256, (lw * lh * 4,), dtype=torch.uint8).numpy(), lw, lh)
+            try:
+                lg(c, tight(vc_get_linesize(W, c) * H, 4 if c == 6 else 2 if c == 27 else 1), W, H, x, y)
+            except RuntimeError:  # the span passes the row's end: refused
+                pass
+            lg.close()
+            n += 1
+    for w, h in ((8, 1), (24, 7), (1920, 3)):
+        for full in (0, 1):
+            r12 = tight(vc_get_linesize(w, 6) * h, 4)
+            y416 = api.r12l_to_y416_fake(r12, w, h, full, dst=tight(8 * w * h, 2))
+            api.y416_to_r12l_fake(y416, w, h, full, dst=tight(vc_get_linesize(w, 6) * h, 4))
+            api.y416_to_r12l_fake(y416, w, h, full, pitch=vc_get_linesize(w, 6) + 3, dst=tight((h - 1) * (vc_get_linesize(w, 6) + 3) + vc_get_linesize(w, 6), 4))
+            n += 3
 torch.cuda.synchronize()
 print("exercised", n, "calls")

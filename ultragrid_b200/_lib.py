@@ -108,6 +108,11 @@ SIGNATURES = {
     "ugb200_cf_split": (_i, [_i, _i, _i, _i, _i, _vp, ctypes.POINTER(_vp), _vp]),
     "ugb200_pp_border": (_i, [_i, _i, _i, ctypes.POINTER(ctypes.c_uint8), ctypes.c_uint, ctypes.c_uint, _vp, _vp, _vp]),
     "ugb200_pp_interlaced_3d": (_i, [_i, _i, _i, _vp, _vp, _vp, _vp]),
+    "ugb200_cf_logo_create": (_vp, [ctypes.POINTER(ctypes.c_uint8), ctypes.c_uint, ctypes.c_uint]),
+    "ugb200_cf_logo_destroy": (None, [_vp]),
+    "ugb200_cf_logo": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
+    "ugb200_cf_r12l_to_y416_fake": (_i, [_i, _i, _i, _vp, _vp, _vp]),
+    "ugb200_pp_y416_to_r12l_fake": (_i, [_i, _i, _i, _vp, _vp, _sz, _vp]),
     # include/ugb200_jpeg.h
     "ugb200_jpeg_default_params": (None, [_vp]),
     "ugb200_jpeg_encoder_create": (_vp, [_vp]),

@@ -344,6 +344,52 @@ def interlaced_3d(codec, left, right, width, height, dst=None, stream=None):
     _check(rc, "ugb200_pp_interlaced_3d")
     return dst
 
+class logo:
+    """logo:<file>[:<x>[:<y>]] (src/capture_filter/logo.c): the module state's RGBA logo (h x w x 4 uint8, as
+    load_logo_data_from_file leaves it), copied to the device once"""
+
+    def __init__(self, rgba, width, height):
+        buf = bytes(rgba)
+        if len(buf) != width * height * 4:
+            raise ValueError("the logo is width * height RGBA pixels")
+        self.width, self.height = width, height
+        self._h = _L.ugb200_cf_logo_create((ctypes.c_uint8 * len(buf)).from_buffer_copy(buf), width, height)
+        if not self._h:
+            raise RuntimeError("ugb200_cf_logo_create failed")
+
+    def __call__(self, codec, frame, width, height, x=-1, y=-1, stream=None):
+        """blends the logo into `frame` in place; x, y = -1 is the default, bottom right"""
+        rc = _L.ugb200_cf_logo(self._h, int(codec), width, height, x, y, _ptr(frame), _stream(stream))
+        _check(rc, f"ugb200_cf_logo({codec})")
+        return frame
+
+    def close(self):
+        if self._h:
+            _L.ugb200_cf_logo_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+
+def r12l_to_y416_fake(src, width, height, full_range=False, dst=None, stream=None):
+    """r12l_to_y416_fake[:full-range] (src/capture_filter/r12l_to_y416_fake.c): tight R12L -> tight Y416"""
+    dst = _cf_out(src, vc_get_linesize(width, Codec.Y416) * height, dst)
+    rc = _L.ugb200_cf_r12l_to_y416_fake(width, height, int(bool(full_range)), _ptr(src), _ptr(dst), _stream(stream))
+    _check(rc, "ugb200_cf_r12l_to_y416_fake")
+    return dst
+
+
+def y416_to_r12l_fake(src, width, height, full_range=False, pitch=0, dst=None, stream=None):
+    """y416_to_r12l_fake[:full-range] (src/vo_postprocess/y416_to_r12l_fake.c): tight Y416 -> R12L rows at `pitch`
+    (0: vc_get_linesize(width, R12L))"""
+    pitch = pitch or vc_get_linesize(width, Codec.R12L)
+    dst = _cf_out(src, pitch * height, dst)
+    rc = _L.ugb200_pp_y416_to_r12l_fake(width, height, int(bool(full_range)), _ptr(src), _ptr(dst), pitch, _stream(stream))
+    _check(rc, "ugb200_pp_y416_to_r12l_fake")
+    return dst
+
+
 class AvPlanes(ctypes.Structure):
     """struct ugb200_av_planes (include/ugb200_lavc.h): AVFrame::data / AVFrame::linesize"""
     _fields_ = [("data", ctypes.c_void_p * 4), ("linesize", ctypes.c_int * 4)]
