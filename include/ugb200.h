@@ -319,6 +319,32 @@ UGB_API int ugb200_cf_r12l_to_y416_fake(int width, int height, int full_range, c
 UGB_API int ugb200_pp_y416_to_r12l_fake(int width, int height, int full_range, const void *src, void *dst, size_t pitch,
                                         cuda_wrapper_stream_t stream);
 
+/* ---- resize (src/capture_filter/resize.c; capture filter and, through its wrapper, postprocessor) ------------------
+ * The resampling is not the reference's bytes (it runs in OpenCV): it follows the exact integer / float32 contract
+ * of DESIGN.md §2 "Resize", modelled on OpenCV's generic path.  Everything resize.c itself decides (route, output
+ * codec and size, letterbox) is the reference's.  Frames are tight (vc_get_linesize pitch; I420 as three planes).
+ * The handle keeps the tables of the last input descriptor and, for codecs outside the resize set, a staging frame
+ * in the route codec; calls on one handle must be ordered (one stream, or synchronised).  Every refusal writes
+ * nothing. */
+/* the module's struct resize_param values: mode 1 = fraction (factor), 2 = dimensions (tw, th); algo = cv::INTER_*
+ * (0 nearest, 1 linear, 2 cubic, 3 area, 4 lanczos4) or -1 (RESIZE_ALGO_DFL: linear).  NULL on other values, a
+ * factor that is not finite and > 0, or tw / th <= 0. */
+typedef struct ugb200_cf_resize *ugb200_cf_resize_t;
+UGB_API ugb200_cf_resize_t ugb200_cf_resize_create(int mode, double factor, int tw, int th, int algo);
+UGB_API void ugb200_cf_resize_destroy(ugb200_cf_resize_t r);
+/* out[0..7]: route codec (the input codec if in {RGB, RGBA, I420, UYVY, YUYV, RG48}, else get_best_decoder_from over
+ * that set), out codec (RG48 for a 16-bit route, else RGB), out_w, out_h (fraction: (int) (w * factor); dimensions:
+ * tw, th), the resampled rectangle x, y, w, h (resize_utils.cpp's letterbox; the whole frame in fraction mode).
+ * Returns 0, -1 (null handle, size <= 0, an output or rectangle of size 0, an odd width on a UYVY / YUYV route, an
+ * odd width or height on I420) or -4 (no route; cubic, lanczos4, or area at other than integer downscales). */
+UGB_API int ugb200_cf_resize_geometry(ugb200_cf_resize_t r, int codec, int width, int height, int out[8]);
+/* filter() of one tile into `dst` (vc_get_linesize(out_w, out codec) * out_h bytes, every one written: margins 0).
+ * Codecs outside the resize set are first converted to the route codec (ugb200_pixfmt_convert) into the handle's
+ * staging frame on `stream`.  0, -1 (also: null pointers, dst overlapping src), -2 (launch or device allocation
+ * failure) or -4 as ugb200_cf_resize_geometry. */
+UGB_API int ugb200_cf_resize(ugb200_cf_resize_t r, int codec, int width, int height, const void *src, void *dst,
+                             cuda_wrapper_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -342,5 +342,25 @@ if ONLY not in ("jpeg", "staged"):
             api.y416_to_r12l_fake(y416, w, h, full, dst=tight(vc_get_linesize(w, 6) * h, 4))
             api.y416_to_r12l_fake(y416, w, h, full, pitch=vc_get_linesize(w, 6) + 3, dst=tight((h - 1) * (vc_get_linesize(w, 6) + 3) + vc_get_linesize(w, 6), 4))
             n += 3
+    # resize on tight buffers: every native layout at odd and even sizes (odd ones refused on 4:2:x routes), each
+    # algorithm, down- and upscales, a letterboxed and a pillarboxed target, and the staged v210 route
+    for c in (12, 1, 2, 3, 29, 27):
+        for w, h in ((2, 2), (3, 5), (47, 3), (96, 54), (131, 7)):
+            nb = w * h + 2 * ((w + 1) // 2) * ((h + 1) // 2) if c == 29 else vc_get_linesize(w, c) * h
+            for kw in (dict(factor=0.5), dict(factor=1.5, algo="nearest"), dict(factor=0.5, algo="area"), dict(size=(40, 10)),
+                       dict(size=(9, 30), algo="nearest")):
+                r = api.Resize(**kw)
+                try:
+                    _, oc, ow, oh, _ = r.geometry(c, w, h)
+                    r(tight(nb, 1), c, w, h, dst=tight(vc_get_linesize(ow, oc) * oh, 3))
+                except RuntimeError:  # odd sizes on 4:2:x routes, empty outputs, area where it is not built
+                    pass
+                r.close()
+                n += 1
+    r = api.Resize(factor=0.5)
+    for w, h in ((48, 6), (50, 7), (1920, 3)):
+        r(tight(vc_get_linesize(w, 7) * h), 7, w, h, dst=tight(vc_get_linesize(w // 2, 27) * (h // 2)))
+        n += 1
+    r.close()
 torch.cuda.synchronize()
 print("exercised", n, "calls")

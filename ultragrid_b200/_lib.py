@@ -113,6 +113,10 @@ SIGNATURES = {
     "ugb200_cf_logo": (_i, [_vp, _i, _i, _i, _i, _i, _vp, _vp]),
     "ugb200_cf_r12l_to_y416_fake": (_i, [_i, _i, _i, _vp, _vp, _vp]),
     "ugb200_pp_y416_to_r12l_fake": (_i, [_i, _i, _i, _vp, _vp, _sz, _vp]),
+    "ugb200_cf_resize_create": (_vp, [_i, ctypes.c_double, _i, _i, _i]),
+    "ugb200_cf_resize_destroy": (None, [_vp]),
+    "ugb200_cf_resize_geometry": (_i, [_vp, _i, _i, _i, ctypes.POINTER(_i)]),
+    "ugb200_cf_resize": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
     # include/ugb200_jpeg.h
     "ugb200_jpeg_default_params": (None, [_vp]),
     "ugb200_jpeg_encoder_create": (_vp, [_vp]),

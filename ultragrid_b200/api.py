@@ -390,6 +390,58 @@ def y416_to_r12l_fake(src, width, height, full_range=False, pitch=0, dst=None, s
     return dst
 
 
+RESIZE_ALGOS = {"nearest": 0, "linear": 1, "cubic": 2, "area": 3, "lanczos4": 4}  # cv::INTER_* (resize_utils.cpp)
+
+
+class Resize:
+    """resize:<num>[/<den>] | resize:<w>x<h> [:algo=<a>] (src/capture_filter/resize.c): a handle holding the module's
+    resize_param and, per input descriptor, the resampling tables and the route's staging frame.  factor= or size=
+    (tw, th); algo a name of RESIZE_ALGOS, a cv::INTER_* value, or None / -1 for the default (linear)."""
+
+    def __init__(self, factor=None, size=None, algo="linear"):
+        if (factor is None) == (size is None):
+            raise ValueError("give factor or size")
+        a = -1 if algo is None else RESIZE_ALGOS[algo] if isinstance(algo, str) else int(algo)
+        tw, th = size if size is not None else (0, 0)
+        self._h = _L.ugb200_cf_resize_create(1 if size is None else 2, float(factor or 0), int(tw), int(th), a)
+        if not self._h:
+            raise ValueError("ugb200_cf_resize_create refused the parameters")
+
+    def geometry(self, codec, width, height):
+        """(route codec, out codec, out_w, out_h, (rect x, y, w, h)); RuntimeError with the code on a refusal"""
+        out = (ctypes.c_int * 8)()
+        _check(_L.ugb200_cf_resize_geometry(self._h, int(codec), width, height, out), "ugb200_cf_resize_geometry")
+        return Codec(out[0]), Codec(out[1]), out[2], out[3], tuple(out[4:8])
+
+    def __call__(self, src, codec, width, height, dst=None, stream=None):
+        """(dst, out codec, out_w, out_h): dst allocated (zeroed) when None"""
+        out = (ctypes.c_int * 8)()
+        rc = _L.ugb200_cf_resize_geometry(self._h, int(codec), width, height, out)
+        if rc == 0 and dst is None:
+            dst = torch.zeros(vc_get_linesize(out[2], Codec(out[1])) * out[3], dtype=torch.uint8, device=src.device)
+        if rc == 0:
+            rc = _L.ugb200_cf_resize(self._h, int(codec), width, height, _ptr(src), _ptr(dst), _stream(stream))
+        _check(rc, f"ugb200_cf_resize({codec})")
+        return dst, Codec(out[1]), out[2], out[3]
+
+    def close(self):
+        if self._h:
+            _L.ugb200_cf_resize_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        self.close()
+
+
+def resize(src, codec, width, height, factor=None, size=None, algo="linear", dst=None, stream=None):
+    """one frame through a fresh Resize handle: (dst, out_codec, out_w, out_h)"""
+    r = Resize(factor, size, algo)
+    try:
+        return r(src, codec, width, height, dst=dst, stream=stream)
+    finally:
+        r.close()
+
+
 class AvPlanes(ctypes.Structure):
     """struct ugb200_av_planes (include/ugb200_lavc.h): AVFrame::data / AVFrame::linesize"""
     _fields_ = [("data", ctypes.c_void_p * 4), ("linesize", ctypes.c_int * 4)]

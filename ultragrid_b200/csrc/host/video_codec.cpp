@@ -18,7 +18,7 @@ struct info_t {
 const info_t infos[] = {
         { RGBA, "RGBA", 4, 1, 1, 8, true, SUBS_4444 }, { UYVY, "UYVY", 4, 2, 2, 8, false, SUBS_422 },  { YUYV, "YUYV", 4, 2, 2, 8, false, SUBS_422 },
         { VUYA, "VUYA", 4, 1, 1, 8, false, SUBS_4444 }, { R10k, "R10k", 4, 1, 64, 10, true, SUBS_444 }, { R12L, "R12L", 36, 8, 8, 12, true, SUBS_444 },
-        { v210, "v210", 16, 6, 48, 10, false, SUBS_422 }, { DXT1, "DXT1", 1, 2, 0, 2, true, SUBS_UNKNOWN }, { DXT5, "DXT5", 1, 1, 0, 4, false, SUBS_UNKNOWN },
+        { v210, "v210", 16, 6, 48, 10, false, SUBS_422 }, { UGB_DVS10, "DVS10", 16, 6, 48, 10, false, SUBS_422 }, { DXT1, "DXT1", 1, 2, 0, 2, true, SUBS_UNKNOWN }, { DXT5, "DXT5", 1, 1, 0, 4, false, SUBS_UNKNOWN },
         { RGB, "RGB", 3, 1, 1, 8, true, SUBS_444 },      { JPEG, "JPEG", 1, 1, 0, 8, false, SUBS_UNKNOWN }, { BGR, "BGR", 3, 1, 1, 8, true, SUBS_444 },
         { RG48, "RG48", 6, 1, 1, 16, true, SUBS_444 },   { I420, "I420", 3, 2, 2, 8, false, SUBS_420 },     { Y216, "Y216", 8, 2, 2, 16, false, SUBS_422 },
         { Y416, "Y416", 8, 1, 1, 16, false, SUBS_4444 },
