@@ -331,12 +331,17 @@ UGB_API int ugb200_pp_y416_to_r12l_fake(int width, int height, int full_range, c
  * factor that is not finite and > 0, or tw / th <= 0. */
 typedef struct ugb200_cf_resize *ugb200_cf_resize_t;
 UGB_API ugb200_cf_resize_t ugb200_cf_resize_create(int mode, double factor, int tw, int th, int algo);
+/* The same parameters and NULL cases.  Its handles also resample with cubic, lanczos4, and area at ratios that are
+ * not integer downscales (area upscaling included), each to the contract of DESIGN.md §2 "Resize"; nearest, linear
+ * and integer area give the bytes of a ugb200_cf_resize_create handle.  -4 from them means only "no route". */
+UGB_API ugb200_cf_resize_t ugb200_cf_resize_create2(int mode, double factor, int tw, int th, int algo);
 UGB_API void ugb200_cf_resize_destroy(ugb200_cf_resize_t r);
 /* out[0..7]: route codec (the input codec if in {RGB, RGBA, I420, UYVY, YUYV, RG48}, else get_best_decoder_from over
  * that set), out codec (RG48 for a 16-bit route, else RGB), out_w, out_h (fraction: (int) (w * factor); dimensions:
  * tw, th), the resampled rectangle x, y, w, h (resize_utils.cpp's letterbox; the whole frame in fraction mode).
  * Returns 0, -1 (null handle, size <= 0, an output or rectangle of size 0, an odd width on a UYVY / YUYV route, an
- * odd width or height on I420) or -4 (no route; cubic, lanczos4, or area at other than integer downscales). */
+ * odd width or height on I420) or -4 (no route; on a ugb200_cf_resize_create handle also cubic, lanczos4, or area
+ * at other than integer downscales). */
 UGB_API int ugb200_cf_resize_geometry(ugb200_cf_resize_t r, int codec, int width, int height, int out[8]);
 /* filter() of one tile into `dst` (vc_get_linesize(out_w, out codec) * out_h bytes, every one written: margins 0).
  * Codecs outside the resize set are first converted to the route codec (ugb200_pixfmt_convert) into the handle's

@@ -362,5 +362,32 @@ if ONLY not in ("jpeg", "staged"):
         r(tight(vc_get_linesize(w, 7) * h), 7, w, h, dst=tight(vc_get_linesize(w // 2, 27) * (h // 2)))
         n += 1
     r.close()
+    # ugb200_cf_resize_create2: cubic, lanczos4, generic area and area upscaling on every native layout, then the
+    # staged v210 route; source and output each exactly as long as their frames, at offsets 1 and 3
+    all_kw = (dict(factor=0.5, algo="cubic"), dict(factor=0.3, algo="cubic"), dict(factor=0.75, algo="lanczos4"),
+              dict(factor=0.1, algo="lanczos4"), dict(factor=1.5, algo="lanczos4"), dict(factor=2 / 3, algo="area"),
+              dict(factor=1.5, algo="area"), dict(size=(40, 10), algo="cubic"), dict(size=(9, 30), algo="area"))
+    for c in (12, 1, 2, 3, 29, 27):
+        for w, h in ((1, 1), (2, 2), (3, 5), (47, 3), (131, 7)):
+            nb = w * h + 2 * ((w + 1) // 2) * ((h + 1) // 2) if c == 29 else vc_get_linesize(w, c) * h
+            for kw in all_kw:
+                r = api.Resize(all_algos=True, **kw)
+                try:
+                    _, oc, ow, oh, _ = r.geometry(c, w, h)
+                    r(tight(nb, 1), c, w, h, dst=tight(vc_get_linesize(ow, oc) * oh, 3))
+                except RuntimeError:  # odd sizes on 4:2:x routes, empty outputs
+                    pass
+                r.close()
+                n += 1
+    for kw in all_kw[:7]:
+        r = api.Resize(all_algos=True, **kw)
+        for w, h in ((48, 6), (50, 7), (1920, 3)):
+            try:
+                _, oc, ow, oh, _ = r.geometry(7, w, h)
+                r(tight(vc_get_linesize(w, 7) * h), 7, w, h, dst=tight(vc_get_linesize(ow, oc) * oh))
+            except RuntimeError:  # empty outputs (factor 0.1 of a few rows)
+                pass
+            n += 1
+        r.close()
 torch.cuda.synchronize()
 print("exercised", n, "calls")

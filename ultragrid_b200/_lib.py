@@ -114,6 +114,7 @@ SIGNATURES = {
     "ugb200_cf_r12l_to_y416_fake": (_i, [_i, _i, _i, _vp, _vp, _vp]),
     "ugb200_pp_y416_to_r12l_fake": (_i, [_i, _i, _i, _vp, _vp, _sz, _vp]),
     "ugb200_cf_resize_create": (_vp, [_i, ctypes.c_double, _i, _i, _i]),
+    "ugb200_cf_resize_create2": (_vp, [_i, ctypes.c_double, _i, _i, _i]),
     "ugb200_cf_resize_destroy": (None, [_vp]),
     "ugb200_cf_resize_geometry": (_i, [_vp, _i, _i, _i, ctypes.POINTER(_i)]),
     "ugb200_cf_resize": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),

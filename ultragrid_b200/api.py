@@ -396,14 +396,16 @@ RESIZE_ALGOS = {"nearest": 0, "linear": 1, "cubic": 2, "area": 3, "lanczos4": 4}
 class Resize:
     """resize:<num>[/<den>] | resize:<w>x<h> [:algo=<a>] (src/capture_filter/resize.c): a handle holding the module's
     resize_param and, per input descriptor, the resampling tables and the route's staging frame.  factor= or size=
-    (tw, th); algo a name of RESIZE_ALGOS, a cv::INTER_* value, or None / -1 for the default (linear)."""
+    (tw, th); algo a name of RESIZE_ALGOS, a cv::INTER_* value, or None / -1 for the default (linear).  all_algos=True
+    creates through ugb200_cf_resize_create2, whose handles also build cubic, lanczos4 and area at any ratio."""
 
-    def __init__(self, factor=None, size=None, algo="linear"):
+    def __init__(self, factor=None, size=None, algo="linear", all_algos=False):
         if (factor is None) == (size is None):
             raise ValueError("give factor or size")
         a = -1 if algo is None else RESIZE_ALGOS[algo] if isinstance(algo, str) else int(algo)
         tw, th = size if size is not None else (0, 0)
-        self._h = _L.ugb200_cf_resize_create(1 if size is None else 2, float(factor or 0), int(tw), int(th), a)
+        create = _L.ugb200_cf_resize_create2 if all_algos else _L.ugb200_cf_resize_create
+        self._h = create(1 if size is None else 2, float(factor or 0), int(tw), int(th), a)
         if not self._h:
             raise ValueError("ugb200_cf_resize_create refused the parameters")
 
@@ -433,9 +435,9 @@ class Resize:
         self.close()
 
 
-def resize(src, codec, width, height, factor=None, size=None, algo="linear", dst=None, stream=None):
+def resize(src, codec, width, height, factor=None, size=None, algo="linear", dst=None, stream=None, all_algos=False):
     """one frame through a fresh Resize handle: (dst, out_codec, out_w, out_h)"""
-    r = Resize(factor, size, algo)
+    r = Resize(factor, size, algo, all_algos)
     try:
         return r(src, codec, width, height, dst=dst, stream=stream)
     finally:
