@@ -47,7 +47,9 @@ UGB_API int ugb200_uyvy_to_dxt6_async(const void *src, void *out, int size_x, in
  * with decoder = get_decoder_from_to(in, out)  (src/pixfmt_conv.h:62-63, src/pixfmt_conv.c:3110-3125,
  * row loop as tools/convert.cpp:148-152).  Per-row results are byte-identical to the reference decoder,
  * including how many bytes of dst_len each loop really writes.  src_size = readable bytes from src
- * (0 = src_pitch*height): some reference loops over-read a partial pixel group; reads past src_size give 0. */
+ * (0 = src_pitch*height): some reference loops over-read a partial pixel group; reads past src_size give 0.  The plain copies
+ * (in == out, and RGB -> RGB / RGBA -> RGBA with the default shifts 0, 8, 16) follow the same rule: nothing past src_size is read, and
+ * the bytes of dst_len that would come from there are written as 0. */
 UGB_API int ugb200_pixfmt_supported(int in_codec, int out_codec); /* get_decoder_from_to() != NULL */
 UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *dst, long dst_pitch, const void *src, long src_pitch,
                           int dst_len, int height, long src_size, int rshift, int gshift, int bshift,

@@ -37,6 +37,9 @@ def lavc_cpu(orc, ref_cpu, in_codec, fmt, src, w, h, pad=0):
     from ultragrid_b200 import api
     shapes = api.av_plane_shapes(fmt, w, h, pad)
     bufs, p, ls = planes_for(shapes)
+    for n in ("orc_lavc_v210", "orc_lavc_uyvy", "orc_lavc_gbrp"):  # pointers must not go through ctypes' default int conversion
+        getattr(orc, n).argtypes, getattr(orc, n).restype = [_i, _vp, _i, _i, _vp, _vp], None
+    orc.orc_lavc_rgb.argtypes, orc.orc_lavc_rgb.restype = [_i, _i, _i, _vp, _vp, _i, _i, _vp, _vp], None
     if in_codec == V210:
         orc.orc_lavc_v210({"YUV420P10LE": 0, "YUV422P10LE": 1, "YUV444P10LE": 2, "YUV444P16LE": 3}[fmt], src.ctypes.data, w, h, p, ls)
     elif in_codec == UYVY:

@@ -1152,12 +1152,37 @@ static int launch_line(void *dst, long dst_pitch, const void *src, long src_pitc
         return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
-static int copy_rows(void *dst, long dst_pitch, const void *src, long src_pitch, int len, int height, cudaStream_t s)
+/// rows [row0, height) of copy_rows, byte by byte: reads past src_total give 0 (include/ugb200.h)
+__global__ void __launch_bounds__(256) copy_rows_tail_kernel(uint8_t *__restrict__ dst, long dst_pitch, const uint8_t *__restrict__ src, long src_pitch, int len,
+                                                             int row0, int height, long src_total)
+{
+        const long n = (long) (height - row0) * len;
+        for (long i = blockIdx.x * (long) blockDim.x + threadIdx.x; i < n; i += (long) gridDim.x * blockDim.x) {
+                const long row = row0 + i / len, x = i % len, a = row * src_pitch + x;
+                dst[row * dst_pitch + x] = a < src_total ? src[a] : 0;
+        }
+}
+
+/// vc_memcpy over the rows: the rows that lie inside src_size in one cudaMemcpy2DAsync, the rest (where the source ends) by copy_rows_tail_kernel
+static int copy_rows(void *dst, long dst_pitch, const void *src, long src_pitch, int len, int height, long src_size, cudaStream_t s)
 {
         if (len <= 0 || height <= 0) {
                 return 0;
         }
-        return cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, len, height, cudaMemcpyDeviceToDevice, s) == cudaSuccess ? 0 : -2;
+        if (src_size <= 0) {
+                src_size = src_pitch * height;
+        }
+        const long whole = src_size < len ? 0 : (src_size - len) / src_pitch + 1 < height ? (src_size - len) / src_pitch + 1 : height;
+        if (whole > 0 && cudaMemcpy2DAsync(dst, dst_pitch, src, src_pitch, len, whole, cudaMemcpyDeviceToDevice, s) != cudaSuccess) {
+                return -2;
+        }
+        if (whole == height) {
+                return 0;
+        }
+        const long n = (height - whole) * (long) len, blocks = (n + 255) / 256;
+        copy_rows_tail_kernel<<<(int) (blocks < 4096 ? blocks : 4096), 256, 0, s>>>((uint8_t *) dst, dst_pitch, (const uint8_t *) src, src_pitch, len, (int) whole,
+                                                                                  height, src_size);
+        return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
 }  // namespace ugb
@@ -1277,7 +1302,7 @@ extern "C" UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *
                 return -1;
         }
         if (in_codec == out_codec && out_codec != UGB_RGBA && out_codec != UGB_RGB) {
-                return copy_rows(dst, dst_pitch, src, src_pitch, dst_len, height, s);  // vc_memcpy (pixfmt_conv.c:2529-2536)
+                return copy_rows(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, s);  // vc_memcpy (pixfmt_conv.c:2529-2536)
         }
         const bool dfl_shift = rshift == 0 && gshift == 8 && bshift == 16;
         switch (in_codec * 256 + out_codec) {
@@ -1306,12 +1331,12 @@ extern "C" UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *
                 return launch_line<conv_rgba_rgb>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, conv_params{ 0, 8, 16, conv_rgba_rgb::aux(dst_len) }, s);
         case UGB_RGBA * 256 + UGB_RGBA:
                 if (dfl_shift) {
-                        return copy_rows(dst, dst_pitch, src, src_pitch, dst_len, height, s);  // pixfmt_conv.c:546-547
+                        return copy_rows(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, s);  // pixfmt_conv.c:546-547
                 }
                 return launch_line<conv_rgba_rgba>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_RGB * 256 + UGB_RGB:
                 if (dfl_shift) {
-                        return copy_rows(dst, dst_pitch, src, src_pitch, dst_len, height, s);  // pixfmt_conv.c:740-741
+                        return copy_rows(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, s);  // pixfmt_conv.c:740-741
                 }
                 return launch_line<conv_rgb_rgb>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_UYVY * 256 + UGB_v210:
