@@ -21,7 +21,7 @@ for algo in (T.DF, T.BOB, T.LINEAR, 3):
         for w, h in ((5, 4), (21, 5)):
             for call in ((0, 1) if algo != 3 else (0,)):
                 for d in ((0, 1) if algo == T.DF else (0,)):
-                    L = T.linesize(w, c)
+                    L = T.vc_get_linesize(w, c)
                     fill = 0xA5 if n % 2 else 0x00
                     pitch = L + (8 if n % 3 else 0)
                     prev, cur = util.rng_bytes(L * h, 2000 + n), util.rng_bytes(L * h, 3000 + n)

@@ -72,8 +72,7 @@ def _bind(lib):
 
 
 def ref_lib():
-    path = os.path.join(util.ORACLE_DIR, "_ref", "libcolour_filters_ref.so")
-    return _bind(ctypes.CDLL(path)) if os.path.exists(path) else None
+    return util.ref_lib("libcolour_filters_ref.so", _bind)
 
 
 @pytest.fixture(scope="module")
@@ -312,12 +311,6 @@ def test_mutants_fail(ref, name):
 
 
 # ---- CPU: the golden fixtures (the reference where it is not built) ---------------------------------------------
-def _golden():
-    if not os.path.exists(GOLDEN):
-        pytest.skip("golden fixtures absent")
-    return np.load(GOLDEN)
-
-
 def golden_outputs(g):
     """[(case, got, mask)] from the fixtures: `got` holds the bytes the reference wrote, mask covers them"""
     out = []
@@ -335,7 +328,7 @@ def golden_outputs(g):
 
 
 def test_restatement_equals_golden():
-    g = _golden()
+    g = util.golden(GOLDEN)
     cpus_of = {}
     for case, got, mask in golden_outputs(g):
         # gamma's written length carries the reference's task count; derive it back
@@ -357,7 +350,7 @@ def test_restatement_equals_golden():
 
 @pytest.mark.parametrize("name", list(MUTANTS))
 def test_mutants_fail_golden(name):
-    outputs = [(c, got, mask) for c, got, mask in golden_outputs(_golden()) if c[0] != "gamma" and (c[5] >= 900 or c[5] < 0)]
+    outputs = [(c, got, mask) for c, got, mask in golden_outputs(util.golden(GOLDEN)) if c[0] != "gamma" and (c[5] >= 900 or c[5] < 0)]
     assert _mutant_fails(name, outputs, 1), f"mutant {name} still equals the reference"
 
 
@@ -369,36 +362,6 @@ def test_header_constant_matches():
 
 
 # ---- GPU --------------------------------------------------------------------------------------------------------
-def _dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-class Guarded:
-    """a device buffer of n bytes at byte offset `off` inside a sentinel-filled allocation"""
-
-    def __init__(self, n, off=0, fill=0x5A, data=None):
-        import torch
-        self.pad, self.off, self.n, self.fill = 256, off, n, fill
-        self.buf = torch.full((n + 2 * self.pad + 16,), fill, dtype=torch.uint8, device="cuda")
-        if data is not None:
-            self.view.copy_(_dev(data))
-
-    @property
-    def view(self):
-        a = self.pad + self.off
-        return self.buf[a:a + self.n]
-
-    def host(self):
-        return self.buf.cpu().numpy()
-
-    def check_outside(self):
-        h = self.host()
-        a = self.pad + self.off
-        assert (h[:a] == self.fill).all() and (h[a + self.n:] == self.fill).all(), "wrote outside the buffer"
-        return h[a:a + self.n]
-
-
 def stream_model(f, c, w, h, param, src):
     """the contract form: what ugb200_cf_* write over their output frame (None where the frame byte is untouched),
     computed in slices of 48 * 65536 bytes (a whole number of units of every codec)"""
@@ -420,8 +383,8 @@ def stream_model(f, c, w, h, param, src):
 def run_gpu(f, c, w, h, param, src, src_off=0, dst_off=0, stream=None):
     from ultragrid_b200 import api
     n = out_len(f, c, w, h, param)
-    s = Guarded(src.size, src_off, 0x33, src)
-    d = Guarded(n, dst_off, 0xC3)
+    s = util.Guarded(src.size, src_off, 0x33, src)
+    d = util.Guarded(n, dst_off, 0xC3)
     if f == "matrix":
         api.matrix(c, s.view, w, h, MATRICES[param[0]], param[1], dst=d.view, stream=stream)
     elif f == "matrix2":
@@ -495,7 +458,7 @@ def test_gpu_gamma_tables():
             w = (1 << ib) // 3 + 1
             src = np.zeros(linesize(w, c), np.uint8)
             src[:ramp.size] = ramp
-            out = g(c, _dev(src), w, 1, ob).cpu().numpy()
+            out = g(c, util.dev(src), w, 1, ob).cpu().numpy()
             got = out.view(np.uint8 if ob == 8 else np.uint16)[:1 << ib]
             assert np.array_equal(got, t[(ib, ob)]), f"gamma {gv} table {(ib, ob)}"
         g.close()
@@ -510,7 +473,7 @@ def test_gpu_matrix2_v210_equals_composed_route():
     for w, h, mi in ((47, 3, 1), (48, 5, 3), (131, 7, 8), (1918, 1081, 2), (7680, 4320, 1)):
         src = src_frame(v210, w, h, 40_000 + w)
         n = src.size
-        s = _dev(src)
+        s = util.dev(src)
         fused = api.matrix2(v210, s, w, h, MATRICES[mi]).cpu().numpy()
         W = n // 16 * 6
         y416 = api.pixfmt_convert(Codec.v210, Codec.Y416, s, W, 1)

@@ -16,6 +16,7 @@ import pytest
 import field_rate_ref as F
 import interlace_ref as IR
 import util
+from ultragrid_b200.codec import vc_get_linesize
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "field_rate_golden.npz")
 FILLS = (0x00, 0xA5)
@@ -23,11 +24,6 @@ CODECS = (IR.UYVY, IR.RGB, IR.RGBA, IR.I420, IR.DVS10, IR.RG48, IR.Y216, IR.Y416
 WIDTHS = (1, 2, 3, 5, 7, 8, 13, 47, 49, 100, 131)
 HEIGHTS = (2, 3, 4, 5, 6, 7)
 DF, BOB, LINEAR = 0, 1, 2
-
-
-def linesize(w, c):
-    from ultragrid_b200.codec import vc_get_linesize
-    return vc_get_linesize(w, c)
 
 
 # ---- the reference ---------------------------------------------------------------------------------------------
@@ -43,8 +39,7 @@ def _bind(lib):
 
 
 def ref_lib():
-    path = os.path.join(util.ORACLE_DIR, "_ref", "libfield_rate_ref.so")
-    return _bind(ctypes.CDLL(path)) if os.path.exists(path) else None
+    return util.ref_lib("libfield_rate_ref.so", _bind)
 
 
 @pytest.fixture(scope="module")
@@ -77,7 +72,7 @@ class Slack:
 
 def ref_run(ref, algo, c, w, h, call, prev, cur, dst, pitch, d=0):
     """perform_* on harness copies; returns (dst bytes of the frame, dst bytes around it)"""
-    L = linesize(w, c)
+    L = vc_get_linesize(w, c)
     row = max(L, pitch)
     p, q, o = Slack(prev, row, 0x5A), Slack(cur, row, 0x5A), Slack(dst, row, fill=int(dst[0]) if dst.size else 0)
     if algo == 3:
@@ -128,7 +123,7 @@ def test_restatement_equals_reference(ref, algo):
     for a, c, w, h, call, d in cases():
         if a != algo:
             continue
-        L = linesize(w, c)
+        L = vc_get_linesize(w, c)
         prev, cur = inputs(L, h, n)
         n += 1
         for pad in (0, 20):
@@ -147,7 +142,7 @@ def test_restatement_equals_reference(ref, algo):
                                           (3, IR.UYVY, 1920)])
 @pytest.mark.parametrize("h", (1080, 1081))
 def test_restatement_equals_reference_full_frames(ref, algo, codec, w, h):
-    L = linesize(w, codec)
+    L = vc_get_linesize(w, codec)
     prev, cur = inputs(L, h, w + h)
     for call in ((0, 1) if algo != 3 else (0,)):
         for d in ((0, 1) if algo == DF else (0,)):
@@ -180,7 +175,7 @@ def test_module_sequence_pins_the_call_and_buffer_model(ref):
     """init / reconfigure / getf / postprocess of the module itself over f1..f5, both calls each, `nodelay`"""
     for algo in (DF, BOB, LINEAR):
         for c, w, h in ((IR.UYVY, 24, 7), (IR.UYVY, 40, 8), (IR.v210, 48, 6), (IR.v210, 96, 9)):
-            L = linesize(w, c)
+            L = vc_get_linesize(w, c)
             frames = [util.rng_bytes(L * h, 40 + i + algo) for i in range(5)]
             pitch = L + 8
             out = np.full(2 * 5 * pitch * h, 0x77, np.uint8)
@@ -199,7 +194,7 @@ def test_module_sequence_pins_the_call_and_buffer_model(ref):
 
 def test_interlace_sequence_pins_the_buffer_model(ref):
     for c, w, h in ((IR.UYVY, 24, 7), (IR.v210, 48, 6)):
-        L = linesize(w, c)
+        L = vc_get_linesize(w, c)
         frames = [util.rng_bytes(L * h, 60 + i) for i in range(4)]
         out = np.zeros(2 * L * h, np.uint8)
         assert ref.ref_interlace_sequence(c, w, h, np.concatenate(frames).ctypes.data, 4, out.ctypes.data, L) == 2
@@ -215,7 +210,7 @@ def test_reference_writes_outside_the_frame_only_where_listed(ref):
     for algo, c, w, h, call, d in cases():
         if w not in (5, 47) or h not in (4, 5):
             continue
-        L = linesize(w, c)
+        L = vc_get_linesize(w, c)
         prev, cur = inputs(L, h, w + h)
         pitch = L + 20
         dst = np.zeros(pitch * h, np.uint8)
@@ -291,7 +286,7 @@ def test_mutant_avg_lines_fails(ref, name, codec, mutant):
 
 def test_mutant_row_rules_fail(ref):
     c, w = IR.UYVY, 8
-    L = linesize(w, c)
+    L = vc_get_linesize(w, c)
     # quirk 6: at odd h a "fixed" double_framerate would fill row h-1 from cur
     h = 5
     prev, cur = inputs(L, h, 3)
@@ -314,7 +309,7 @@ def test_mutant_row_rules_fail(ref):
 
 # ---- golden fixtures (made from the reference by tests/golden/make_field_rate_golden.py) -------------------------
 def test_restatement_equals_golden():
-    g = np.load(GOLDEN)
+    g = util.golden(GOLDEN)
     n = 0
     for k in g.files:
         if not k.endswith("_meta"):
@@ -334,26 +329,13 @@ GUARD = 64
 SENT = 0x3C
 
 
-def _framed(content, offset=0):
-    import torch
-    buf = torch.full((2 * GUARD + offset + content.size,), SENT, dtype=torch.uint8, device="cuda")
-    buf[GUARD + offset:GUARD + offset + content.size] = torch.from_numpy(content).cuda()
-    return buf, GUARD + offset
-
-
-def _check_guards(host, start, n):
-    assert (host[:start] == SENT).all() and (host[start + n:] == SENT).all(), "a byte outside the buffer changed"
-
-
 def gpu_run(algo, c, L, h, call, prev, cur, dst_init, pitch, d=0, offset=0):
     """ugb200_pp_* between sentinels; returns (rc, dst bytes)"""
     import torch
     from ultragrid_b200 import _lib, api
     lib = _lib.load()
-    p, po = _framed(prev, offset)
-    q, qo = _framed(cur, offset)
-    o, oo = _framed(dst_init, offset)
-    P, Q, O = (ctypes.c_void_p(t.data_ptr() + off) for t, off in ((p, po), (q, qo), (o, oo)))
+    p, q, o = (util.Guarded(a.size, offset, SENT, a, GUARD) for a in (prev, cur, dst_init))
+    P, Q, O = (ctypes.c_void_p(g.view.data_ptr()) for g in (p, q, o))
     st = api._stream()
     if algo == DF:
         rc = lib.ugb200_pp_double_framerate(c, P, Q, L, h, call, d, O, pitch, st)
@@ -364,12 +346,9 @@ def gpu_run(algo, c, L, h, call, prev, cur, dst_init, pitch, d=0, offset=0):
     else:
         rc = lib.ugb200_pp_interlace(Q, P, L, h, O, pitch, st)
     torch.cuda.synchronize()
-    ph, qh, oh = p.cpu().numpy(), q.cpu().numpy(), o.cpu().numpy()
-    for hb, off, src in ((ph, po, prev), (qh, qo, cur)):
-        _check_guards(hb, off, src.size)
-        assert np.array_equal(hb[off:off + src.size], src), "a source changed"
-    _check_guards(oh, oo, dst_init.size)
-    return rc, oh[oo:oo + dst_init.size]
+    for g, src in ((p, prev), (q, cur)):
+        assert np.array_equal(g.check_outside(), src), "a source changed"
+    return rc, o.check_outside()
 
 
 def _align(algo, c, d):
@@ -385,7 +364,7 @@ def test_gpu_exact(algo):
     for a, c, w, h, call, d in cases():
         if a != algo:
             continue
-        L = linesize(w, c)
+        L = vc_get_linesize(w, c)
         for pad, off in ((0, 0), (20, 0), (6, 1)):
             for fill in FILLS:
                 _check_gpu(algo, c, L, h, call, d, pad, off, fill, n)
@@ -433,7 +412,7 @@ def test_gpu_exact_raw_line_sizes(codec):
                                        (IR.RG48, 3840, 2160), (IR.R10k, 7680, 4321), (IR.R12L, 3840, 2160), (IR.R12L, 7680, 4320),
                                        (IR.UYVY, 1920, 1081)])
 def test_gpu_frames(codec, w, h):
-    L = linesize(w, codec)
+    L = vc_get_linesize(w, codec)
     prev, cur = inputs(L, h, w + h)
     dst = np.full(L * h, 0xA5, np.uint8)
     for algo in (DF, BOB, LINEAR, 3):
@@ -453,7 +432,7 @@ def test_gpu_fused_d_equals_weave_then_deinterlace_ex(codec):
     import torch
     from ultragrid_b200 import api
     al = 4 if codec in (IR.v210, IR.R10k, IR.R12L) else 2 if IR.BITS[codec] == 16 else 1
-    shapes = [(linesize(w, codec), h) for w, h in ((1920, 1080), (1918, 1081), (100, 7), (47, 5))]
+    shapes = [(vc_get_linesize(w, codec), h) for w, h in ((1920, 1080), (1918, 1081), (100, 7), (47, 5))]
     shapes += [(L, h) for L in (68, 136, 188, 112, 260, 1004) if L % al == 0 for h in (4, 5)]
     for L, h in shapes:
         prev, cur = inputs(L, h, L + h)
@@ -477,7 +456,7 @@ def test_gpu_fused_d_equals_weave_then_deinterlace_ex(codec):
 def test_gpu_side_stream_and_api():
     import torch
     from ultragrid_b200 import api
-    L, h = linesize(1920, IR.UYVY), 1080
+    L, h = vc_get_linesize(1920, IR.UYVY), 1080
     prev, cur = inputs(L, h, 5)
     s = torch.cuda.Stream()
     P, Q = torch.from_numpy(prev).cuda(), torch.from_numpy(cur).cuda()
@@ -540,7 +519,7 @@ def test_gpu_refusals_write_nothing():
 
 @pytest.mark.gpu
 def test_gpu_matches_golden():
-    g = np.load(GOLDEN)
+    g = util.golden(GOLDEN)
     for k in g.files:
         if not k.endswith("_meta"):
             continue

@@ -47,8 +47,7 @@ def _bind(lib):
 
 
 def ref_lib():
-    path = os.path.join(util.ORACLE_DIR, "_ref", "libgeometry_filters_ref.so")
-    return _bind(ctypes.CDLL(path)) if os.path.exists(path) else None
+    return util.ref_lib("libgeometry_filters_ref.so", _bind)
 
 
 @pytest.fixture(scope="module")
@@ -331,12 +330,6 @@ def golden_cases():
     return [c for i, c in enumerate(cases()) if R.linesize(c[2], c[1]) * c[3] <= 4000 and i % 8 == 0]
 
 
-def _golden():
-    if not os.path.exists(GOLDEN):
-        pytest.skip("golden fixtures absent")
-    return np.load(GOLDEN, allow_pickle=False)
-
-
 def golden_key(case):
     f, c, w, h, p, seed = case
     return f"{f}_{c}_{w}x{h}_s{seed}"
@@ -353,7 +346,7 @@ def golden_run(g, case):
 
 
 def test_restatement_equals_golden():
-    g = _golden()
+    g = util.golden(GOLDEN)
     cs = golden_cases()
     assert all(f"{golden_key(c)}_0_out" in g.files for c in cs), "fixtures out of date: run tests/golden/make_geometry_filters_golden.py"
     for case in cs:
@@ -362,39 +355,12 @@ def test_restatement_equals_golden():
 
 @pytest.mark.parametrize("name", list(MUTANTS))
 def test_mutants_fail_golden(name):
-    g = _golden()
+    g = util.golden(GOLDEN)
     cs = [c for c in golden_cases() if MUTANTS[name][1](c)]
     assert any(check_fails(case, golden_run(g, case), **MUTANTS[name][0]) for case in cs), f"mutant {name} still equals the reference"
 
 
 # ---- GPU --------------------------------------------------------------------------------------------------------
-def _dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-class Guarded:
-    """a device buffer of n bytes at byte offset `off` inside a sentinel-filled allocation"""
-
-    def __init__(self, n, off=0, fill=0x5A, data=None):
-        import torch
-        self.pad, self.off, self.n, self.fill = 256, off, n, fill
-        self.buf = torch.full((n + 2 * self.pad + 16,), fill, dtype=torch.uint8, device="cuda")
-        if data is not None:
-            self.view.copy_(_dev(data))
-
-    @property
-    def view(self):
-        a = self.pad + self.off
-        return self.buf[a:a + self.n]
-
-    def check_outside(self):
-        h = self.buf.cpu().numpy()
-        a = self.pad + self.off
-        assert (h[:a] == self.fill).all() and (h[a + self.n:] == self.fill).all(), "wrote outside the buffer"
-        return h[a:a + self.n]
-
-
 def frame_len(case):
     """the output frame of each buffer: what the device may write"""
     f, c, w, h, p, seed = case
@@ -424,8 +390,8 @@ def run_gpu(case, src_off=0, dst_off=0, stream=None):
     from ultragrid_b200 import api
     f, c, w, h, p, seed = case
     src = frame(c, w, h, seed)
-    s = Guarded(src.size, src_off, 0x33, src)
-    outs = [Guarded(n, dst_off, 0xC3) for n in frame_len(case)]
+    s = util.Guarded(src.size, src_off, 0x33, src)
+    outs = [util.Guarded(n, dst_off, 0xC3) for n in frame_len(case)]
     d = outs[0].view
     if f == "flip":
         api.flip(c, s.view, w, h, dst=d, stream=stream)
@@ -440,7 +406,7 @@ def run_gpu(case, src_off=0, dst_off=0, stream=None):
         api.border(c, s.view, w, h, color, bw, bh, dst=d, stream=stream)
     else:
         right = frame(c, w, h, seed + 1)
-        r = Guarded(right.size, (src_off * 7) % 16, 0x44, right)
+        r = util.Guarded(right.size, (src_off * 7) % 16, 0x44, right)
         api.interlaced_3d(c, s.view, r.view, w, h, dst=d, stream=stream)
         torch.cuda.synchronize()
         assert np.array_equal(r.check_outside(), right), "the right tile changed"
@@ -519,11 +485,11 @@ def test_gpu_round_trips():
     from ultragrid_b200 import api
     for c, w, h in ((UYVY, 1921, 1081), (v210, 1920, 1080), (RGB, 131, 7)):
         src = frame(c, w, h, 77)
-        s = _dev(src)
+        s = util.dev(src)
         assert np.array_equal(api.flip(c, api.flip(c, s, w, h), w, h).cpu().numpy(), src)
     for c, w, h, x, y in ((v210, 1920, 1080, 4, 4), (RGB, 1920, 1080, 3, 2), (R12L, 960, 540, 2, 2), (R10k, 640, 480, 5, 3)):
         src = frame(c, w, h, 78)
-        tiles = [t.cpu().numpy() for t in api.split(c, _dev(src), w, h, x, y)]
+        tiles = [t.cpu().numpy() for t in api.split(c, util.dev(src), w, h, x, y)]
         L, tl, n = R.linesize(w, c), R.linesize(w // x, c), int((w // x) * R.bpp(c))
         offs = R.split_offsets(c, w, x)
         merged = np.zeros((h, L), np.uint8)

@@ -13,6 +13,7 @@ import pytest
 
 import interlace_ref as R
 import util
+from ultragrid_b200.codec import vc_get_linesize
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "interlace_golden.npz")
 FILLS = (0x00, 0xA5)
@@ -20,11 +21,6 @@ WIDTHS = (1, 2, 3, 5, 6, 7, 47, 48, 1918, 1920)
 RAW_LS = (14, 17, 44, 52, 100, 172, 300, 1004)  # not multiples of 16, 36 or 128
 LINES = (1, 2, 3, 4, 5, 6, 7)
 LEGACY_LS = (16, 17, 31, 36, 40, 52, 3840, 5760, 23040)
-
-
-def linesize(w, c):
-    from ultragrid_b200.codec import vc_get_linesize
-    return vc_get_linesize(w, c)
 
 
 def _bind(lib):
@@ -74,7 +70,7 @@ def ref_legacy(ref, data, L, lines, offset):
 def ex_cases():
     """(codec, L, lines, pitch pad) for every non-opaque codec: codec widths, raw line sizes, lines 1-7"""
     for c in R.NON_OPAQUE:
-        sizes = sorted({linesize(w, c) for w in WIDTHS} | set(RAW_LS))
+        sizes = sorted({vc_get_linesize(w, c) for w in WIDTHS} | set(RAW_LS))
         for L in sizes:
             for lines in LINES:
                 yield c, L, lines, 0 if lines % 2 else 20
@@ -127,7 +123,7 @@ def test_ex_restatement_equals_reference(ref, codec):
 @pytest.mark.parametrize("codec,w", [(R.UYVY, 1920), (R.v210, 1920), (R.RG48, 1918), (R.R12L, 1920), (R.R10k, 1918)])
 @pytest.mark.parametrize("lines", (1080, 1081))
 def test_ex_full_frames_equal_reference(ref, codec, w, lines):
-    L = linesize(w, codec)
+    L = vc_get_linesize(w, codec)
     src = util.rng_bytes(L * lines, w + lines)
     for fill in FILLS:
         dst = np.full(L * lines, fill, np.uint8)
@@ -150,7 +146,7 @@ def written(c, L, lines, pitch, contract):
     return (a == b), a
 
 
-@pytest.mark.parametrize("codec,L", [(R.RG48, linesize(1918, R.RG48)), (R.Y216, 1004), (R.Y416, 172), (R.R12L, linesize(1920, R.R12L)),
+@pytest.mark.parametrize("codec,L", [(R.RG48, vc_get_linesize(1918, R.RG48)), (R.Y216, 1004), (R.Y416, 172), (R.R12L, vc_get_linesize(1920, R.R12L)),
                                      (R.R12L, 36 * 7 + 8), (R.R12L, 36 * 6), (R.v210, 1004), (R.UYVY, 1918 * 2)])
 def test_deliberate_differences_are_exactly_the_quirk_list(codec, L):
     lines, pitch = 5, L + 12
@@ -225,12 +221,8 @@ def test_il_round_trip_is_identity():
 
 
 # ---- golden fixtures (made from the reference by tests/golden/make_interlace_golden.py) ------------------------
-def golden():
-    return np.load(GOLDEN)
-
-
 def test_restatement_equals_golden():
-    g = golden()
+    g = util.golden(GOLDEN)
     n = 0
     for k in g.files:
         if k.endswith("_meta"):
@@ -256,43 +248,19 @@ GUARD = 64
 SENT = 0x3C
 
 
-def _dev(host):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(host)).cuda()
-
-
-def _framed(content, offset=0):
-    """a device buffer: GUARD sentinel bytes, `offset` more, content, GUARD sentinel bytes"""
-    import torch
-    buf = torch.full((2 * GUARD + offset + content.size,), SENT, dtype=torch.uint8, device="cuda")
-    buf[GUARD + offset:GUARD + offset + content.size] = torch.from_numpy(content).cuda()
-    return buf, GUARD + offset
-
-
-def _check_guards(host, start, n):
-    assert (host[:start] == SENT).all() and (host[start + n:] == SENT).all(), "a byte outside the buffer changed"
-
-
 def gpu_ex(codec, src, L, dst_init, pitch, lines, in_place=False):
     """ugb200_vc_deinterlace_ex between sentinels; returns (rc, dst bytes)"""
     from ultragrid_b200 import _lib, api
     import torch
     lib = _lib.load()
-    s, so = _framed(src)
-    if in_place:
-        d, do = s, so
-    else:
-        d, do = _framed(dst_init)
-    rc = lib.ugb200_vc_deinterlace_ex(codec, ctypes.c_void_p(s.data_ptr() + so), L, ctypes.c_void_p(d.data_ptr() + do), pitch, lines,
-                                      api._stream())
+    s = util.Guarded(src.size, 0, SENT, src, GUARD)
+    d = s if in_place else util.Guarded(dst_init.size, 0, SENT, dst_init, GUARD)
+    rc = lib.ugb200_vc_deinterlace_ex(codec, ctypes.c_void_p(s.view.data_ptr()), L, ctypes.c_void_p(d.view.data_ptr()), pitch, lines, api._stream())
     torch.cuda.synchronize()
-    sh, dh = s.cpu().numpy(), d.cpu().numpy()
-    n = src.size if in_place else dst_init.size
-    _check_guards(dh, do, n)
+    got = d.check_outside()
     if not in_place:
-        _check_guards(sh, so, src.size)
-        assert np.array_equal(sh[so:so + src.size], src), "source changed"
-    return rc, dh[do:do + n]
+        assert np.array_equal(s.check_outside(), src), "source changed"
+    return rc, got
 
 
 @pytest.mark.gpu
@@ -335,7 +303,7 @@ def test_gpu_ex_exact(codec):
                                        (R.R12L, 1920, 1080), (R.R10k, 1918, 1081), (R.Y216, 1920, 1080), (R.RGB, 3840, 2160),
                                        (R.UYVY, 7680, 4320), (R.R12L, 3840, 2161), (R.v210, 7680, 4320)])
 def test_gpu_ex_frames(codec, w, h):
-    L = linesize(w, codec)
+    L = vc_get_linesize(w, codec)
     src = util.rng_bytes(L * h, w + h)
     dst = np.full(L * h, 0xA5, np.uint8)
     rc, got = gpu_ex(codec, src, L, dst, L, h)
@@ -354,11 +322,11 @@ def test_gpu_ex_frames(codec, w, h):
 def test_gpu_ex_side_stream_and_api():
     import torch
     from ultragrid_b200 import api
-    L, h = linesize(1920, R.UYVY), 1080
+    L, h = vc_get_linesize(1920, R.UYVY), 1080
     src = util.rng_bytes(L * h, 5)
     want = R.deinterlace_ex(R.UYVY, src, L, np.zeros(L * h, np.uint8), L, h, contract=True)
     s = torch.cuda.Stream()
-    t = _dev(src)
+    t = util.dev(src)
     torch.cuda.synchronize()
     with torch.cuda.stream(s):
         out = api.deinterlace_ex(R.UYVY, t, L, h, stream=s)
@@ -414,16 +382,15 @@ def test_gpu_legacy_exact():
                 continue
             for off in (0, 1, 4):
                 data = util.rng_bytes(L * lines, L * 7 + lines + off)
-                buf, o = _framed(data, off)
-                assert lib.ugb200_vc_deinterlace(ctypes.c_void_p(buf.data_ptr() + o), L, lines, api._stream()) == 0
+                buf = util.Guarded(data.size, off, SENT, data, GUARD)
+                assert lib.ugb200_vc_deinterlace(ctypes.c_void_p(buf.view.data_ptr()), L, lines, api._stream()) == 0
                 torch.cuda.synchronize()
-                h = buf.cpu().numpy()
-                _check_guards(h, o, data.size)
+                got = buf.check_outside()
                 want = R.deinterlace(data, L, lines)
-                assert np.array_equal(h[o:o + data.size], want), (L, lines, off, np.flatnonzero(h[o:o + data.size] != want)[:8])
+                assert np.array_equal(got, want), (L, lines, off, np.flatnonzero(got != want)[:8])
                 if ref is not None and lines < 1080:
                     assert np.array_equal(want, ref_legacy(ref, data, L, lines, off))
-    assert lib.ugb200_vc_deinterlace(ctypes.c_void_p(buf.data_ptr() + GUARD), 15, 8, api._stream()) == -1
+    assert lib.ugb200_vc_deinterlace(ctypes.c_void_p(buf.buf.data_ptr() + GUARD), 15, 8, api._stream()) == -1
 
 
 @pytest.mark.gpu
@@ -431,7 +398,7 @@ def test_gpu_legacy_exact():
 def test_gpu_legacy_frames(w, h, bpp):
     from ultragrid_b200 import api
     data = util.rng_bytes(w * bpp * h, w)
-    t = _dev(data)
+    t = util.dev(data)
     api.deinterlace(t, w * bpp, h)
     assert np.array_equal(t.cpu().numpy(), R.deinterlace(data, w * bpp, h))
 
@@ -448,16 +415,14 @@ def test_gpu_il_exact(name):
             src = util.rng_bytes(L * h, L + h)
             want = getattr(R, name)(src, L, h)
             for off in (0, 1, 4):
-                s, so = _framed(src, off)
-                d, do = _framed(np.zeros(L * h, np.uint8), 0)
-                assert fn(ctypes.c_void_p(d.data_ptr() + do), ctypes.c_void_p(s.data_ptr() + so), L, h, api._stream()) == 0
-                assert fn(ctypes.c_void_p(s.data_ptr() + so), ctypes.c_void_p(s.data_ptr() + so), L, h, api._stream()) == 0
+                s = util.Guarded(src.size, off, SENT, src, GUARD)
+                d = util.Guarded(L * h, 0, SENT, np.zeros(L * h, np.uint8), GUARD)
+                sp, dp = ctypes.c_void_p(s.view.data_ptr()), ctypes.c_void_p(d.view.data_ptr())
+                assert fn(dp, sp, L, h, api._stream()) == 0
+                assert fn(sp, sp, L, h, api._stream()) == 0
                 torch.cuda.synchronize()
-                dh, sh = d.cpu().numpy(), s.cpu().numpy()
-                _check_guards(dh, do, src.size)
-                _check_guards(sh, so, src.size)
-                assert np.array_equal(dh[do:do + src.size], want), (name, L, h, off)
-                assert np.array_equal(sh[so:so + src.size], want), ("in place", name, L, h, off)
+                assert np.array_equal(d.check_outside(), want), (name, L, h, off)
+                assert np.array_equal(s.check_outside(), want), ("in place", name, L, h, off)
     buf = torch.zeros(4096, dtype=torch.uint8, device="cuda")
     assert fn(ctypes.c_void_p(buf.data_ptr() + 16), ctypes.c_void_p(buf.data_ptr()), 64, 8, api._stream()) == -1  # partial overlap
     assert (buf == 0).all()
@@ -469,7 +434,7 @@ def test_gpu_il_round_trip_on_a_side_stream():
     from ultragrid_b200 import api
     for L, h in ((3840, 1080), (7680 * 2, 4321), (5, 7)):
         src = util.rng_bytes(L * h, h)
-        t = _dev(src)
+        t = util.dev(src)
         torch.cuda.synchronize()
         s = torch.cuda.Stream()
         with torch.cuda.stream(s):
@@ -485,7 +450,7 @@ def test_gpu_il_round_trip_on_a_side_stream():
 def test_gpu_matches_golden():
     import torch
     from ultragrid_b200 import api
-    g = golden()
+    g = util.golden(GOLDEN)
     for k in g.files:
         if not k.endswith("_meta"):
             continue
@@ -498,17 +463,17 @@ def test_gpu_matches_golden():
                 continue  # the reference leaves those tails unwritten; checked against the restatement above
             if (c in (R.v210, R.R10k) and (L % 4 or pitch % 4)):
                 continue
-            dst = _dev(np.full(pitch * lines, fill, np.uint8))
-            api.deinterlace_ex(c, _dev(src), L, lines, dst=dst, dst_pitch=pitch)
+            dst = util.dev(np.full(pitch * lines, fill, np.uint8))
+            api.deinterlace_ex(c, util.dev(src), L, lines, dst=dst, dst_pitch=pitch)
             assert np.array_equal(dst.cpu().numpy(), want), p
         elif kind == 1:
             L, lines = meta[:2]
-            t = _dev(src)
+            t = util.dev(src)
             api.deinterlace(t, L, lines)
             assert np.array_equal(t.cpu().numpy(), want), p
         else:
             L, h = meta[:2]
-            t = _dev(src)
+            t = util.dev(src)
             (api.il_upper_to_merged if kind == 2 else api.il_merged_to_upper)(t, L, h)
             torch.cuda.synchronize()
             assert np.array_equal(t.cpu().numpy(), want), p

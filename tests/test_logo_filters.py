@@ -57,8 +57,7 @@ def _bind(lib):
 
 
 def ref_lib():
-    path = os.path.join(util.ORACLE_DIR, "_ref", "liblogo_filters_ref.so")
-    return _bind(ctypes.CDLL(path)) if os.path.exists(path) else None
+    return util.ref_lib("liblogo_filters_ref.so", _bind)
 
 
 @pytest.fixture(scope="module")
@@ -407,12 +406,6 @@ def golden_key(case):
     return "_".join(str(v) for v in case)
 
 
-def _golden():
-    if not os.path.exists(GOLDEN):
-        pytest.skip("golden fixtures absent")
-    return np.load(GOLDEN, allow_pickle=False)
-
-
 def golden_data(ref):
     """what the fixtures hold: the reference's outputs for the golden cases"""
     out = {}
@@ -437,7 +430,7 @@ def _golden_y416(g, case):
 
 
 def test_restatement_equals_golden():
-    g = _golden()
+    g = util.golden(GOLDEN)
     cs = golden_logo_cases()
     assert len(cs) > 100 and all(f"logo_{golden_key(c)}_a" in g.files for c in cs), "fixtures out of date: run tests/golden/make_logo_filters_golden.py"
     for case in cs:
@@ -451,7 +444,7 @@ def test_restatement_equals_golden():
 
 @pytest.mark.parametrize("name", list(LOGO_MUTANTS) + ["c_scale_13"])
 def test_mutants_fail_golden(name):
-    g = _golden()
+    g = util.golden(GOLDEN)
     if name == "c_scale_13":
         case = golden_fake_cases()[3]
         with pytest.raises(AssertionError):
@@ -463,33 +456,6 @@ def test_mutants_fail_golden(name):
 
 
 # ---- GPU --------------------------------------------------------------------------------------------------------
-def _dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
-class Guarded:
-    """a device buffer of n bytes at byte offset `off` inside a sentinel-filled allocation"""
-
-    def __init__(self, n, off=0, fill=0x5A, data=None):
-        import torch
-        self.pad, self.off, self.n, self.fill = 256, off, n, fill
-        self.buf = torch.full((n + 2 * self.pad + 16,), fill, dtype=torch.uint8, device="cuda")
-        if data is not None:
-            self.view.copy_(_dev(data))
-
-    @property
-    def view(self):
-        a = self.pad + self.off
-        return self.buf[a:a + self.n]
-
-    def check_outside(self):
-        h = self.buf.cpu().numpy()
-        a = self.pad + self.off
-        assert (h[:a] == self.fill).all() and (h[a + self.n:] == self.fill).all(), "wrote outside the buffer"
-        return h[a:a + self.n]
-
-
 def gpu_logo_check(case, off=0, stream=None):
     """the frame after the call equals the restatement's everywhere: its span, and nothing else, is written"""
     import torch
@@ -498,7 +464,7 @@ def gpu_logo_check(case, off=0, stream=None):
     f = frame(c, W, H, seed)
     rgba = logo_rgba(w, h, alpha, seed)
     want = R.logo(c, f, W, H, rgba, x, y)
-    g = Guarded(f.size, off, 0xC3, f)
+    g = util.Guarded(f.size, off, 0xC3, f)
     lg = api.logo(rgba.reshape(-1), w, h)
     if want is None:
         with pytest.raises(RuntimeError, match="code -1"):
@@ -547,13 +513,13 @@ def _fake_gpu(case, src_off=0, dst_off=0, stream=None):
     full, w, h, extra, seed = case
     L = R.linesize(w, R12L)
     src = r12l_src(w, h, seed)
-    s = Guarded(src.size, src_off, 0x33, src)
-    d = Guarded(8 * w * h, dst_off, 0xC3)
+    s = util.Guarded(src.size, src_off, 0x33, src)
+    d = util.Guarded(8 * w * h, dst_off, 0xC3)
     api.r12l_to_y416_fake(s.view, w, h, full, dst=d.view, stream=stream)
     ysrc = y416_src(w, h, seed + 1)
-    ys = Guarded(ysrc.size, dst_off, 0x44, ysrc)
+    ys = util.Guarded(ysrc.size, dst_off, 0x44, ysrc)
     pitch = L + extra
-    rd = Guarded((h - 1) * pitch + L, src_off, 0xC3)
+    rd = util.Guarded((h - 1) * pitch + L, src_off, 0xC3)
     api.y416_to_r12l_fake(ys.view, w, h, full, pitch=pitch, dst=rd.view, stream=stream)
     torch.cuda.synchronize()
     assert np.array_equal(s.check_outside(), src) and np.array_equal(ys.check_outside(), ysrc), "a source changed"
@@ -585,7 +551,7 @@ def test_gpu_fake_pair_4k_8k_and_side_stream():
 def test_gpu_fake_pair_8k_round_trip_is_the_identity():
     from ultragrid_b200 import api
     w, h = 7680, 4320
-    src = _dev(r12l_src(w, h, 11))
+    src = util.dev(r12l_src(w, h, 11))
     for full in (False, True):
         back = api.y416_to_r12l_fake(api.r12l_to_y416_fake(src, w, h, full), w, h, full)
         assert bool((back == src).all()), full

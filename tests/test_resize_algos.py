@@ -14,7 +14,7 @@ import pytest
 import resize_algos_ref as A
 import resize_filter_ref as R
 import util
-from test_resize_filter import Guarded, _dev, frame, route_bytes
+from test_resize_filter import frame, route_bytes
 
 RATIOS = [0.5, 1 / 3, 0.75, 2 / 3, 1.5, 2.0, 0.3]
 FRACS = np.linspace(0, 1, 1001, dtype=np.float32)[:-1]
@@ -296,14 +296,14 @@ def gpu_check(param, c, w, h, seed=1, handle=None, stream=None, data=None):
     rc, want = want_for(param, c, w, h, data)
     kw = dict(factor=factor) if mode == R.FRACTION else dict(size=(tw, th))
     r = handle or api.Resize(algo=algo, all_algos=True, **kw)
-    g = Guarded(want.size if rc == 0 else 64)
+    g = util.Guarded(want.size if rc == 0 else 64)
     if rc != 0:
         with pytest.raises(RuntimeError, match=f"code {rc}"):
-            r(_dev(data), c, w, h, dst=g.view, stream=stream)
+            r(util.dev(data), c, w, h, dst=g.view, stream=stream)
         torch.cuda.synchronize()
         assert (g.check_outside() == g.fill).all(), "a refusal wrote"
     else:
-        r(_dev(data), c, w, h, dst=g.view, stream=stream)
+        r(util.dev(data), c, w, h, dst=g.view, stream=stream)
         torch.cuda.synchronize()
         got = g.check_outside()
         assert np.array_equal(got, want), f"{param} codec {c} {w}x{h}: {int(np.count_nonzero(got != want))} bytes differ"
@@ -407,7 +407,7 @@ def test_gpu_built_algorithms_equal_create_handles():
     for algo in ("nearest", "linear", "area"):
         for c, w, h in ((R.RGB, 97, 31), (R.UYVY, 96, 48), (R.I420, 64, 32), (R.RG48, 35, 9)):
             for kw in (dict(factor=0.5), dict(factor=0.25), dict(factor=1.5), dict(size=(40, 40))):
-                src = _dev(frame(c, w, h, w + c))
+                src = util.dev(frame(c, w, h, w + c))
                 outs = []
                 for all_algos in (False, True):
                     try:

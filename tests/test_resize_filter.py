@@ -42,8 +42,7 @@ def _bind(lib):
 
 
 def ref_lib():
-    path = os.path.join(util.ORACLE_DIR, "_ref", "libresize_filter_ref.so")
-    return _bind(ctypes.CDLL(path)) if os.path.exists(path) else None
+    return util.ref_lib("libresize_filter_ref.so", _bind)
 
 
 def ref_parse(ref, cfg):
@@ -184,14 +183,8 @@ def golden_data(ref):
     return out
 
 
-def _golden():
-    if not os.path.exists(GOLDEN):
-        pytest.skip("golden fixtures absent")
-    return np.load(GOLDEN, allow_pickle=False)
-
-
 def test_parse_equals_golden():
-    g = _golden()
+    g = util.golden(GOLDEN)
     for i, cfg in enumerate(PARSE_CORPUS):
         v = g[f"parse_{i}"]
         want = R.parse(cfg)
@@ -201,7 +194,7 @@ def test_parse_equals_golden():
 
 
 def test_route_equals_golden():
-    g = _golden()
+    g = util.golden(GOLDEN)
     for i, case in enumerate(route_cases()):
         v = g[f"route_{i}"]
         check_route(case, None if v[0] == -1 else tuple(int(x) for x in v) + (g[f"route_{i}_bytes"],))
@@ -363,29 +356,6 @@ def test_mutants_fail(name):
 
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------
-class Guarded:
-    """a device buffer of n bytes inside a sentinel-filled allocation"""
-
-    def __init__(self, n, fill=0x5A):
-        import torch
-        self.pad, self.n, self.fill = 256, n, fill
-        self.buf = torch.full((n + 2 * self.pad,), fill, dtype=torch.uint8, device="cuda")
-
-    @property
-    def view(self):
-        return self.buf[self.pad:self.pad + self.n]
-
-    def check_outside(self):
-        h = self.buf.cpu().numpy()
-        assert (h[:self.pad] == self.fill).all() and (h[self.pad + self.n:] == self.fill).all(), "wrote outside the buffer"
-        return h[self.pad:self.pad + self.n]
-
-
-def _dev(a):
-    import torch
-    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
-
-
 def want_for(param, c, w, h, data):
     """the restatement's (code, bytes) for a frame of codec c"""
     from ultragrid_b200 import compress
@@ -401,14 +371,14 @@ def gpu_check(param, c, w, h, seed=1, handle=None, stream=None):
     rc, want = want_for(param, c, w, h, data)
     r = handle or (api.Resize(factor=factor, algo=algo) if mode == R.FRACTION else api.Resize(size=(tw, th), algo=algo))
     n = want.size if rc == 0 else 64
-    g = Guarded(n)
+    g = util.Guarded(n)
     if rc != 0:
         with pytest.raises(RuntimeError, match=f"code {rc}"):
-            r(_dev(data), c, w, h, dst=g.view, stream=stream)
+            r(util.dev(data), c, w, h, dst=g.view, stream=stream)
         torch.cuda.synchronize()
         assert (g.check_outside() == g.fill).all(), "a refusal wrote"
     else:
-        r(_dev(data), c, w, h, dst=g.view, stream=stream)
+        r(util.dev(data), c, w, h, dst=g.view, stream=stream)
         torch.cuda.synchronize()
         got = g.check_outside()
         assert np.array_equal(got, want), f"{param} codec {c} {w}x{h}: {int(np.count_nonzero(got != want))} bytes differ"
@@ -505,9 +475,9 @@ def test_gpu_refusals_write_nothing():
     for param, c, w, h in cases:
         assert gpu_check(param, c, w, h) != 0
     r = api.Resize(factor=0.5)
-    g = Guarded(64)
+    g = util.Guarded(64)
     with pytest.raises(RuntimeError, match="code -4"):  # no route
-        r(_dev(np.zeros(64, np.uint8)), Codec.DXT1, 16, 8, dst=g.view)
+        r(util.dev(np.zeros(64, np.uint8)), Codec.DXT1, 16, 8, dst=g.view)
     buf = torch.zeros(4096, dtype=torch.uint8, device="cuda")
     with pytest.raises(RuntimeError, match="code -1"):  # dst overlapping src
         r(buf[:16 * 8 * 3], Codec.RGB, 16, 8, dst=buf[100:100 + 8 * 4 * 3])

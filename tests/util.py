@@ -172,3 +172,49 @@ def convert_cpu(lib, fn, in_c, out_c, src, width, height, dst_len=None, src_pitc
     rc = getattr(lib, fn)(in_c, out_c, dst.ctypes.data, dst_pitch, srcp.ctypes.data, src_pitch, dst_len, height, *shifts)
     assert rc == 0, rc
     return dst[:dst_pitch * height]
+
+
+# ---- the filter suites' harness ---------------------------------------------------------------------------
+def ref_lib(soname, bind):
+    """oracle/_ref/<soname> with a suite's argument types applied by `bind`, or None when it is not built"""
+    path = os.path.join(ORACLE_DIR, "_ref", soname)
+    return bind(ctypes.CDLL(path)) if os.path.exists(path) else None
+
+
+def golden(path):
+    """the .npz fixtures at `path`, or a skip when they are absent"""
+    if not os.path.exists(path):
+        import pytest
+        pytest.skip("golden fixtures absent")
+    return np.load(path, allow_pickle=False)
+
+
+def dev(a):
+    """a host array copied to the device"""
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a)).cuda()
+
+
+class Guarded:
+    """a device buffer of n bytes (`data`, if given) inside an allocation filled with `fill`: `guard + off` bytes before
+    it, `guard + 16` after it"""
+
+    def __init__(self, n, off=0, fill=0x5A, data=None, guard=256):
+        import torch
+        self.start, self.n, self.fill = guard + off, n, fill
+        self.buf = torch.full((self.start + n + guard + 16,), fill, dtype=torch.uint8, device="cuda")
+        if data is not None:
+            self.view.copy_(dev(data))
+
+    @property
+    def view(self):
+        return self.buf[self.start:self.start + self.n]
+
+    def host(self):
+        return self.buf.cpu().numpy()
+
+    def check_outside(self):
+        """the buffer's bytes, after checking that every byte around them still holds the fill"""
+        h = self.host()
+        assert (h[:self.start] == self.fill).all() and (h[self.start + self.n:] == self.fill).all(), "wrote outside the buffer"
+        return h[self.start:self.start + self.n]

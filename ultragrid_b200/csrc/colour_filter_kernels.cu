@@ -20,6 +20,8 @@
 #include <new>
 
 #include "../../include/ugb200.h"
+#include "filter_args.h"
+#include "host/video_codec.h"
 
 namespace ugb_cf {
 
@@ -285,12 +287,6 @@ __global__ void __launch_bounds__(kThreads) stream_kernel(Op op, const uint8_t *
         }
 }
 
-bool overlap(const void *a, size_t na, const void *b, size_t nb)
-{
-        const uintptr_t x = (uintptr_t) a, y = (uintptr_t) b;
-        return x < y + nb && y < x + na;
-}
-
 template <class Op> int launch(const Op &op, const void *src, size_t in_len, void *dst, size_t out_len, cudaStream_t st)
 {
         const long chunks = long((in_len + Op::IN - 1) / Op::IN);
@@ -298,19 +294,6 @@ template <class Op> int launch(const Op &op, const void *src, size_t in_len, voi
         stream_kernel<Op><<<unsigned((chunks + kThreads - 1) / kThreads), kThreads, 0, st>>>(op, (const uint8_t *) src, (uint8_t *) dst,
                                                                                            long(in_len), long(out_len), chunks, vec);
         return cudaGetLastError() == cudaSuccess ? 0 : -2;
-}
-
-size_t frame_len(int codec, int width, int height)
-{
-        const size_t w = (size_t) width, h = (size_t) height;
-        switch (codec) {
-        case UGB_UYVY: return (w + 1) / 2 * 4 * h;
-        case UGB_RGB: return w * 3 * h;
-        case UGB_RG48: return w * 6 * h;
-        case UGB_Y416: return w * 8 * h;
-        case UGB_v210: return (w + 47) / 48 * 128 * h;
-        default: return 0;
-        }
 }
 
 // ---- gamma -------------------------------------------------------------------------------------------------------
@@ -453,7 +436,7 @@ extern "C" UGB_API int ugb200_cf_gamma(ugb200_cf_gamma_t g, int codec, int out_d
                 return -4;
         }
         const int in_bits = codec == UGB_RGB ? 8 : 16, out_bits = out_depth == 0 ? in_bits : out_depth;
-        const size_t in_len = frame_len(codec, width, height), samples = in_len / (in_bits / 8), out_len = samples * (out_bits / 8);
+        const size_t in_len = vc_get_datalen(width, height, (codec_t) codec), samples = in_len / (in_bits / 8), out_len = samples * (out_bits / 8);
         if ((in_bits == 16 && (uintptr_t) src % 2) || (out_bits == 16 && (uintptr_t) dst % 2) || overlap(src, in_len, dst, out_len)) {
                 return -1;
         }
@@ -478,9 +461,9 @@ extern "C" UGB_API int ugb200_cf_matrix(int codec, int width, int height, const 
         }
         Mat M;
         memcpy(M.m, m, sizeof M.m);
-        const size_t in_len = frame_len(codec, width, height);
+        const size_t in_len = vc_get_datalen(width, height, (codec_t) codec);
         // UYVY -> RGB: the reference writes 6 bytes per 4 over the whole UYVY frame; here output stops at 3 * w * h
-        const size_t out_len = codec == UGB_UYVY ? frame_len(UGB_RGB, width, height) : in_len;
+        const size_t out_len = codec == UGB_UYVY ? vc_get_datalen(width, height, RGB) : in_len;
         if ((codec == UGB_RG48 && ((uintptr_t) src % 2 || (uintptr_t) dst % 2)) || overlap(src, in_len, dst, out_len)) {
                 return -1;
         }
@@ -508,7 +491,7 @@ extern "C" UGB_API int ugb200_cf_matrix2(int codec, int width, int height, const
         }
         Mat M;
         memcpy(M.m, m, sizeof M.m);
-        const size_t len = frame_len(codec, width, height);
+        const size_t len = vc_get_datalen(width, height, (codec_t) codec);
         const unsigned align = codec == UGB_UYVY ? 1 : codec == UGB_Y416 ? 2 : 4;
         if ((uintptr_t) src % align || (uintptr_t) dst % align || overlap(src, len, dst, len)) {
                 return -1;

@@ -17,60 +17,16 @@
 #include <vector>
 
 #include "../../include/ugb200.h"
+#include "filter_args.h"
+#include "host/video_codec.h"
 #include "rgb_to_uyvy.cuh"
-
-namespace ugb_il {
-int scratch_alloc(void **p, size_t n, cudaStream_t st);  // interlace_kernels.cu: stream-ordered scratch
-}
 
 namespace ugb_geo {
 
 constexpr int kThreads = 256;
 
-// ---- codec layout (src/video_codec.c codec_info[]) ------------------------------------------------------------------
-struct Fmt {
-        int bytes, pixels, align;  // block_size_bytes, block_size_pixels, h_align
-        bool block;                // a packed pixel format: crop and split take it (get_pf_block_bytes is meaningful)
-};
-
-Fmt fmt(int codec)
-{
-        switch (codec) {
-        case UGB_RGBA: case UGB_VUYA: return { 4, 1, 1, true };
-        case UGB_UYVY: case UGB_YUYV: return { 4, 2, 2, true };
-        case UGB_R10k: return { 4, 1, 64, true };
-        case UGB_R12L: return { 36, 8, 8, true };
-        case UGB_v210: case UGB_DVS10: return { 16, 6, 48, true };
-        case UGB_RGB: case UGB_BGR: return { 3, 1, 1, true };
-        case UGB_RG48: return { 6, 1, 1, true };
-        case UGB_Y216: return { 8, 2, 2, true };
-        case UGB_Y416: return { 8, 1, 1, true };
-        case UGB_I420: return { 3, 2, 2, false };
-        case UGB_DXT1: case UGB_DXT1_YUV: return { 1, 2, 0, false };
-        case UGB_HW_VDPAU: case UGB_DRM_PRIME: case UGB_VIDEO_CODEC_NONE: return { 0, 0, 0, false };  // no byte layout
-        default: return codec > 0 && codec < UGB_VIDEO_CODEC_COUNT ? Fmt{ 1, 1, 0, false } : Fmt{ 0, 0, 0, false };
-        }
-}
-
-// vc_get_linesize (video_codec.c:507-521)
-long linesize(const Fmt &f, long w)
-{
-        if (f.pixels == 0) {
-                return 0;
-        }
-        if (f.align) {
-                w = (w + f.align - 1) / f.align * f.align;
-        }
-        return (w + f.pixels - 1) / f.pixels * f.bytes;
-}
-
-double bpp(const Fmt &f) { return (double) f.bytes / f.pixels; }  // get_bpp (:309-320)
-
-bool overlap(const void *a, size_t na, const void *b, size_t nb)
-{
-        const uintptr_t x = (uintptr_t) a, y = (uintptr_t) b;
-        return na && nb && x < y + nb && y < x + na;
-}
+// a packed pixel format: crop and split take it (get_pf_block_bytes is meaningful)
+bool packed(codec_t c) { return get_pf_block_bytes(c) > 0 && !is_codec_opaque(c) && !codec_is_planar(c); }
 
 // ---- the row kernel ------------------------------------------------------------------------------------------------
 // Bytes [0, n) of the row at d: byte b is s[b] for b in [c0, c1), else pat[b % period] (border fill).
@@ -306,19 +262,21 @@ struct CropGeom {
         int out_w, out_h, xoff, yoff, xoff_bytes;
 };
 
-int crop_geometry(const Fmt &f, int in_w, int in_h, int width, int height, int xoff, int yoff, CropGeom *g)
+int crop_geometry(codec_t c, int in_w, int in_h, int width, int height, int xoff, int yoff, CropGeom *g)
 {
         // crop_postprocess_reconfigure: MIN in int, then the width rounded to whole blocks in the reference's double arithmetic
         int ow = width ? (width < in_w ? width : in_w) : in_w;
         const int oh = height ? (height < in_h ? height : in_h) : in_h;
-        const int ls = (int) (ow * bpp(f)) / f.bytes * f.bytes;
-        ow = (int) (unsigned) (ls / bpp(f));
+        const double bpp = get_bpp(c);
+        const int bytes = get_pf_block_bytes(c);
+        const int ls = (int) (ow * bpp) / bytes * bytes;
+        ow = (int) (unsigned) (ls / bpp);
         // crop_postprocess: unsigned comparison, so a negative offset is clamped only when the sum wraps
         g->out_w = ow;
         g->out_h = oh;
         g->xoff = (unsigned) xoff + (unsigned) ow > (unsigned) in_w ? in_w - ow : (int) (unsigned) xoff;
         g->yoff = (unsigned) yoff + (unsigned) oh > (unsigned) in_h ? in_h - oh : (int) (unsigned) yoff;
-        g->xoff_bytes = (int) (g->xoff * bpp(f)) / f.bytes * f.bytes;
+        g->xoff_bytes = (int) (g->xoff * bpp) / bytes * bytes;
         return 0;
 }
 
@@ -331,7 +289,7 @@ extern "C" UGB_API int ugb200_cf_flip(int codec, int width, int height, const vo
         if (src == nullptr || dst == nullptr || width <= 0 || height <= 0) {
                 return -1;
         }
-        const long L = linesize(fmt(codec), width);
+        const long L = vc_linesize64(width, (codec_t) codec);
         if (L == 0) {
                 return -4;
         }
@@ -350,7 +308,7 @@ extern "C" UGB_API int ugb200_cf_mirror(int codec, int width, int height, const 
         if (codec != UGB_UYVY) {
                 return -4;
         }
-        const long G = linesize(fmt(codec), width) / 4, groups = G * height;
+        const long G = vc_linesize64(width, (codec_t) codec) / 4, groups = G * height;
         if (overlap(src, 4 * groups, dst, 4 * groups)) {
                 return -1;
         }
@@ -368,12 +326,12 @@ extern "C" UGB_API int ugb200_cf_crop_geometry(int codec, int in_width, int in_h
         if (out == nullptr || in_width <= 0 || in_height <= 0 || width < 0 || height < 0) {
                 return -1;
         }
-        const Fmt f = fmt(codec);
-        if (!f.block) {
+        const codec_t c = (codec_t) codec;
+        if (!packed(c)) {
                 return -4;
         }
         CropGeom g;
-        crop_geometry(f, in_width, in_height, width, height, xoff, yoff, &g);
+        crop_geometry(c, in_width, in_height, width, height, xoff, yoff, &g);
         out[0] = g.out_w, out[1] = g.out_h, out[2] = g.xoff, out[3] = g.yoff;
         return 0;
 }
@@ -384,15 +342,15 @@ extern "C" UGB_API int ugb200_cf_crop(int codec, int in_width, int in_height, in
         if (src == nullptr || in_width <= 0 || in_height <= 0 || width < 0 || height < 0) {
                 return -1;
         }
-        const Fmt f = fmt(codec);
-        if (!f.block) {
+        const codec_t c = (codec_t) codec;
+        if (!packed(c)) {
                 return -4;
         }
         CropGeom g;
-        crop_geometry(f, in_width, in_height, width, height, xoff, yoff, &g);
-        const long src_ls = linesize(f, in_width), src_len = src_ls * in_height;
+        crop_geometry(c, in_width, in_height, width, height, xoff, yoff, &g);
+        const long src_ls = vc_linesize64(in_width, c), src_len = src_ls * in_height;
         if (pitch == 0) {
-                pitch = (size_t) linesize(f, g.out_w);  // the capture filter's vc_get_linesize(out width)
+                pitch = (size_t) vc_linesize64(g.out_w, c);  // the capture filter's vc_get_linesize(out width)
         }
         const long first = (long) g.yoff * src_ls + g.xoff_bytes;
         // an unclamped negative offset makes the first row start before the source
@@ -416,19 +374,19 @@ extern "C" UGB_API int ugb200_cf_split(int codec, int width, int height, int x, 
         if (src == nullptr || tiles == nullptr || width <= 0 || height <= 0 || x <= 0 || y <= 0 || width % x || height % y) {
                 return -1;
         }
-        const Fmt f = fmt(codec);
-        if (!f.block) {
+        const codec_t c = (codec_t) codec;
+        if (!packed(c)) {
                 return -4;
         }
-        const long count = (long) x * y, tw = width / x, th = height / y, L = linesize(f, width), tile_ls = linesize(f, tw);
+        const long count = (long) x * y, tw = width / x, th = height / y, L = vc_linesize64(width, c), tile_ls = vc_linesize64(tw, c);
         // vf_split.cpp:74-81 in the reference's arithmetic: (size_t) (tile_w * bpp) bytes per tile row, the source offset
         // accumulated as `unsigned byte += tile_w * bpp`, truncating at every step
-        const size_t n = (size_t) (tw * bpp(f));
+        const size_t n = (size_t) (tw * get_bpp(c));
         std::vector<uintptr_t> table(count + x);
         unsigned byte = 0u;
         for (long i = 0; i < x; ++i) {
                 table[count + i] = byte;
-                byte += tw * bpp(f);
+                byte += tw * get_bpp(c);
         }
         for (long t = 0; t < count; ++t) {
                 if (tiles[t] == nullptr || overlap(src, (size_t) L * height, tiles[t], (size_t) tile_ls * th)) {
@@ -461,7 +419,7 @@ extern "C" UGB_API int ugb200_pp_border(int codec, int width, int height, const 
         if (codec != UGB_UYVY && codec != UGB_RGB && codec != UGB_RGBA) {
                 return -4;
         }
-        const long L = linesize(fmt(codec), width), bh = border_height;
+        const long L = vc_linesize64(width, (codec_t) codec), bh = border_height;
         long band;  // bytes of each side band
         if (codec == UGB_UYVY) {
                 band = ((long) border_width + 1) / 2 * 4;  // a group at i / 2 * 4 for every even i < width
@@ -488,7 +446,7 @@ extern "C" UGB_API int ugb200_pp_interlaced_3d(int codec, int width, int height,
         if (left == nullptr || right == nullptr || dst == nullptr || width <= 0 || height <= 0) {
                 return -1;
         }
-        const long L = linesize(fmt(codec), width);
+        const long L = vc_linesize64(width, (codec_t) codec);
         if (L == 0) {
                 return -4;
         }

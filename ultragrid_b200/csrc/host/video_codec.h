@@ -4,13 +4,16 @@
 #pragma once
 #include "ug_types.h"
 
+// The layout of every codec id (codec_info[], video_codec.c:120-206); ids outside [NONE, COUNT) have none: sizes 0.
+long vc_linesize64(long width, codec_t codec);                                   // vc_get_linesize without the int overflow
 int vc_get_linesize(unsigned int width, codec_t codec);                          // video_codec.c:507-521
-int vc_get_size(unsigned int width, codec_t codec);                              // :530-538
-size_t vc_get_datalen(unsigned int width, unsigned int height, codec_t codec);   // :543-560
+size_t vc_get_datalen(unsigned int width, unsigned int height, codec_t codec);   // :543-560, in 64 bits
 int get_bits_per_component(codec_t codec);
-bool codec_is_a_rgb(codec_t codec);
+double get_bpp(codec_t codec);
+int get_pf_block_bytes(codec_t codec);
+bool is_codec_opaque(codec_t codec);
+bool codec_is_planar(codec_t codec);                                             // only I420
 const char *get_codec_name(codec_t codec);
-codec_t get_codec_from_name(const char *name);
 struct pixfmt_desc get_pixfmt_desc(codec_t pixfmt);                              // :1134-1143
 int compare_pixdesc(const pixfmt_desc *a, const pixfmt_desc *b, const pixfmt_desc *src);  // :1148-1192
 

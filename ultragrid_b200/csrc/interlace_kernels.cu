@@ -20,6 +20,8 @@
 #include <type_traits>
 
 #include "../../include/ugb200.h"
+#include "filter_args.h"
+#include "host/video_codec.h"
 
 namespace ugb_il {
 
@@ -396,32 +398,11 @@ template <bool TO_MERGED> int il_permute(void *dst_, void *src_, int linesize, i
         return ok ? 0 : -2;
 }
 
-// codec_info[] (video_codec.c:120-206): VCF_OPAQUE and the bits-per-component column
-bool codec_opaque(int c)
-{
-        switch (c) {
-        case UGB_RGBA: case UGB_UYVY: case UGB_YUYV: case UGB_VUYA: case UGB_R10k: case UGB_R12L: case UGB_v210: case UGB_DVS10:
-        case UGB_RGB: case UGB_BGR: case UGB_RG48: case UGB_I420: case UGB_Y216: case UGB_Y416:
-                return false;
-        default:
-                return true;
-        }
-}
-int codec_bpc(int c)
-{
-        switch (c) {
-        case UGB_R10k: case UGB_v210: case UGB_DVS10: return 10;
-        case UGB_R12L: return 12;
-        case UGB_RG48: case UGB_Y216: case UGB_Y416: return 16;
-        default: return 8;
-        }
-}
-
 template <typename Rows>
 int blend_codec(int codec, const Rows &rows, bool in_place, uintptr_t addr, size_t ls, uint8_t *dst, size_t pitch, size_t lines, size_t *blend,
                 cudaStream_t st)
 {
-        const int bpc = codec_bpc(codec);
+        const int bpc = get_bits_per_component((codec_t) codec);
         if (bpc == 8) {
                 *blend = ls;
                 return blend_lanes<K8>(rows, in_place, addr, ls, dst, pitch, lines, *blend, st);
@@ -454,7 +435,7 @@ using namespace ugb_il;
 extern "C" UGB_API int ugb200_vc_deinterlace_ex(int codec, const void *src_, size_t src_linesize, void *dst_, size_t dst_pitch, size_t lines,
                                                 cuda_wrapper_stream_t stream)
 {
-        if (codec <= UGB_VIDEO_CODEC_NONE || codec >= UGB_VIDEO_CODEC_COUNT || codec_opaque(codec)) {
+        if (codec <= UGB_VIDEO_CODEC_NONE || codec >= UGB_VIDEO_CODEC_COUNT || is_codec_opaque((codec_t) codec)) {
                 return -4;
         }
         const uint8_t *src = (const uint8_t *) src_;
@@ -462,7 +443,7 @@ extern "C" UGB_API int ugb200_vc_deinterlace_ex(int codec, const void *src_, siz
         if (!src || !dst || lines == 0 || dst_pitch < src_linesize) {
                 return -1;
         }
-        const int bpc = codec_bpc(codec);
+        const int bpc = get_bits_per_component((codec_t) codec);
         const bool word = codec == UGB_v210 || codec == UGB_R10k || codec == UGB_R12L;
         const uintptr_t align = word ? 4 : bpc == 16 ? 2 : 1;
         if (((uintptr_t) src | (uintptr_t) dst | src_linesize | dst_pitch) % align != 0) {
@@ -470,7 +451,7 @@ extern "C" UGB_API int ugb200_vc_deinterlace_ex(int codec, const void *src_, siz
         }
         const bool in_place = dst == src && dst_pitch == src_linesize;
         const size_t src_end = src_linesize * lines, dst_end = dst_pitch * (lines - 1) + src_linesize;
-        if (!in_place && src_linesize > 0 && dst < src + src_end && src < dst + dst_end) {
+        if (!in_place && overlap(src, src_end, dst, dst_end)) {
                 return -1;
         }
         const cudaStream_t st = (cudaStream_t) stream;
@@ -783,12 +764,6 @@ struct WeaveRows {
         }
 };
 
-bool overlaps(const void *dst, size_t dst_n, const void *src, size_t src_n)
-{
-        const uint8_t *d = (const uint8_t *) dst, *s = (const uint8_t *) src;
-        return s && d < s + src_n && s < d + dst_n;
-}
-
 // the checks every ugb200_pp_* shares: -1 or 0
 int pp_args(const void *a, const void *b, size_t ls, int h, int call, const void *dst, size_t pitch)
 {
@@ -796,13 +771,13 @@ int pp_args(const void *a, const void *b, size_t ls, int h, int call, const void
                 return -1;
         }
         const size_t dst_n = pitch * (size_t) (h - 1) + ls, src_n = ls * (size_t) h;
-        return overlaps(dst, dst_n, a, src_n) || overlaps(dst, dst_n, b, src_n) ? -1 : 0;
+        return overlap(dst, dst_n, a, src_n) || (b && overlap(dst, dst_n, b, src_n)) ? -1 : 0;
 }
 
 // address alignment a codec's samples need (16-bit: 2, packed words: 4)
 size_t codec_align(int codec)
 {
-        return codec == UGB_v210 || codec == UGB_R10k || codec == UGB_R12L ? 4 : codec_bpc(codec) == 16 ? 2 : 1;
+        return codec == UGB_v210 || codec == UGB_R10k || codec == UGB_R12L ? 4 : get_bits_per_component((codec_t) codec) == 16 ? 2 : 1;
 }
 
 }  // namespace ugb_il
@@ -820,7 +795,7 @@ extern "C" UGB_API int ugb200_pp_double_framerate(int codec, const void *prev_, 
                 return call == 0 ? weave<W_DF0>(cur, prev, linesize, dst, pitch, height, linesize, st)
                                  : weave<W_COPY>(cur, nullptr, linesize, dst, pitch, height, linesize, st);
         }
-        if (codec <= UGB_VIDEO_CODEC_NONE || codec >= UGB_VIDEO_CODEC_COUNT || codec_opaque(codec) || codec == UGB_DVS10) {
+        if (codec <= UGB_VIDEO_CODEC_NONE || codec >= UGB_VIDEO_CODEC_COUNT || is_codec_opaque((codec_t) codec) || codec == UGB_DVS10) {
                 return -4;  // what ugb200_vc_deinterlace_ex refuses
         }
         const size_t al = codec_align(codec);
@@ -872,7 +847,7 @@ extern "C" UGB_API int ugb200_pp_linear(int codec, const void *cur_, size_t line
         if (pp_args(cur, nullptr, linesize, height, call, dst, pitch) != 0) {
                 return -1;
         }
-        if (codec <= UGB_VIDEO_CODEC_NONE || codec >= UGB_VIDEO_CODEC_COUNT || codec_opaque(codec)) {
+        if (codec <= UGB_VIDEO_CODEC_NONE || codec >= UGB_VIDEO_CODEC_COUNT || is_codec_opaque((codec_t) codec)) {
                 return -4;
         }
         if (((uintptr_t) cur | (uintptr_t) dst | linesize | pitch) % codec_align(codec) != 0) {
@@ -880,7 +855,7 @@ extern "C" UGB_API int ugb200_pp_linear(int codec, const void *cur_, size_t line
         }
         const cudaStream_t st = (cudaStream_t) stream;
         const size_t L = linesize;
-        const int bpc = codec_bpc(codec);
+        const int bpc = get_bits_per_component((codec_t) codec);
         if (bpc == 8) {
                 return linear_lanes<KH8>(cur, L, dst, pitch, height, call, L, st);
         }

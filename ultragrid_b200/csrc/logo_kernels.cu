@@ -15,6 +15,8 @@
 #include <new>
 
 #include "../../include/ugb200.h"
+#include "filter_args.h"
+#include "host/video_codec.h"
 #include "rgb_line_conv.cuh"
 #include "rgb_to_uyvy.cuh"
 #include "yuv_rgb_conv.cuh"
@@ -24,25 +26,6 @@ namespace ugb_logo {
 using namespace ugb;
 
 constexpr int kThreads = 128;
-
-// codec_info[] (video_codec.c): block bytes (get_pf_block_bytes) and pixels of the five codecs logo.c takes
-struct Fmt {
-        int bytes, pixels;
-};
-
-bool fmt(int codec, Fmt *f)
-{
-        switch (codec) {
-        case UGB_RGB: *f = { 3, 1 }; return true;
-        case UGB_RGBA: *f = { 4, 1 }; return true;
-        case UGB_UYVY: *f = { 4, 2 }; return true;
-        case UGB_RG48: *f = { 6, 1 }; return true;
-        case UGB_R12L: *f = { 36, 8 }; return true;
-        }
-        return false;  // no decoder to or from RGB (get_decoder_from_to() == NULL): logo.c returns its input
-}
-
-long linesize(const Fmt &f, long w) { return (w + f.pixels - 1) / f.pixels * f.bytes; }  // vc_get_linesize (h_align = block pixels here)
 
 long c_div(long a, long b) { return a / b; }  // C truncation toward zero, as logo.c rounds rect_x
 
@@ -297,12 +280,6 @@ __global__ void __launch_bounds__(256) y416_to_r12l_kernel(const uint8_t *__rest
         }
 }
 
-bool overlap(const void *a, size_t na, const void *b, size_t nb)
-{
-        const uintptr_t x = (uintptr_t) a, y = (uintptr_t) b;
-        return na && nb && x < y + nb && y < x + na;
-}
-
 }  // namespace ugb_logo
 
 using namespace ugb_logo;
@@ -354,10 +331,12 @@ extern "C" UGB_API int ugb200_cf_logo(ugb200_cf_logo_t l, int codec, int width, 
         if (l == nullptr || frame == nullptr || width <= 0 || height <= 0) {
                 return -1;
         }
-        Fmt f;
-        if (!fmt(codec, &f)) {
-                return -4;
+        switch (codec) {
+        case UGB_RGB: case UGB_RGBA: case UGB_UYVY: case UGB_RG48: case UGB_R12L: break;
+        default: return -4;  // no decoder to or from RGB (get_decoder_from_to() == NULL): logo.c returns its input
         }
+        const codec_t c = (codec_t) codec;
+        const long bytes = get_pf_block_bytes(c);
         if ((codec == UGB_RG48 && (uintptr_t) frame % 2) || (codec == UGB_R12L && (uintptr_t) frame % 4)) {
                 return -1;
         }
@@ -367,14 +346,14 @@ extern "C" UGB_API int ugb200_cf_logo(ugb200_cf_logo_t l, int codec, int width, 
         if (rect_x < 0 || rect_x + w > width) {
                 rect_x = width - w;
         }
-        rect_x = c_div(rect_x, f.bytes) * f.bytes;  // whole blocks of bytes, counted in pixels
+        rect_x = c_div(rect_x, bytes) * bytes;  // whole blocks of bytes, counted in pixels
         if (rect_y < 0 || rect_y + h > height) {
                 rect_y = height - h;
         }
         if (rect_x < 0 || rect_y < 0) {
                 return 0;  // the reference returns its input untouched
         }
-        const long pitch = linesize(f, width), off = linesize(f, rect_x), span = linesize(f, w);
+        const long pitch = vc_linesize64(width, c), off = vc_linesize64(rect_x, c), span = vc_linesize64(w, c);
         if (off + span > pitch) {
                 return -1;  // the reference writes past the row (into the next one, or past the frame)
         }

@@ -11,6 +11,7 @@
 #include <stdint.h>
 
 #include "../../include/ugb200.h"
+#include "host/video_codec.h"
 
 namespace ugb {
 
@@ -655,7 +656,7 @@ extern "C" UGB_API int ugb200_y216_to_p010le(const struct ugb200_to_planar_data 
         if (!tp_ok(d, 2)) {
                 return -1;
         }
-        const long in_ls = (long) ((d->width + 1) / 2) * 8;  // vc_get_linesize(width, Y216)
+        const long in_ls = vc_linesize64(d->width, Y216);
         const op_y216_p010 op = { d->in_data, in_ls, d->out_data[0], d->out_data[1], d->out_linesize[0], d->out_linesize[1], d->width, d->height,
                                   (d->width + 1 + 3) / 4, (d->height + 1) / 2, tp_vec(d, 2, in_ls) };
         return launch_planar(op, (cudaStream_t) stream);
@@ -677,7 +678,7 @@ extern "C" UGB_API int ugb200_uyvy_to_i420(const struct ugb200_to_planar_data *d
         if (!tp_ok(d, 3)) {
                 return -1;
         }
-        const long in_ls = (long) ((d->width + 1) / 2) * 4;  // vc_get_linesize(width, UYVY)
+        const long in_ls = vc_linesize64(d->width, UYVY);
         const op_uyvy_420<true> op = { d->in_data, in_ls, d->out_data[0], d->out_data[1], d->out_data[2], d->out_linesize[0], d->out_linesize[1], d->out_linesize[2],
                                        d->width, d->height, (d->width + 7) / 8, (d->height + 1) / 2, 0, tp_vec(d, 3, in_ls) };
         return launch_planar(op, (cudaStream_t) stream);
@@ -709,7 +710,7 @@ static int r12l_to_planes(const struct ugb200_to_planar_data *d, int depth, int 
         if (!tp_ok(d, 3) || (d->out_linesize[0] & 1) || (d->out_linesize[1] & 1) || (d->out_linesize[2] & 1)) {
                 return -1;  // asserts of to_planar.c:385-388
         }
-        const long in_ls = (long) ((d->width + 7) / 8) * 36;  // vc_get_linesize(width, R12L)
+        const long in_ls = vc_linesize64(d->width, R12L);
         const op_r12l_gbrp op = { d->in_data, in_ls, { d->out_data[rind], d->out_data[gind], d->out_data[bind] },
                                   { d->out_linesize[rind], d->out_linesize[gind], d->out_linesize[bind] }, d->width, d->height, (d->width + 7) / 8, d->height, depth - 12,
                                   tp_vec(d, 3, 16), (3 & (size_t) d->in_data) == 0 };

@@ -13,6 +13,7 @@
 #include <stdint.h>
 
 #include "../../include/ugb200.h"
+#include "host/video_codec.h"
 
 namespace ugb {
 
@@ -225,7 +226,7 @@ extern "C" int ugb200_v210_to_p010le(const struct ugb200_to_planar_data *d, long
                 return -1;  // asserts of to_planar.c:66-68
         }
         if (in_linesize == 0) {
-                in_linesize = (d->width + 47) / 48 * 128;  // vc_get_linesize(width, v210), video_codec.c:507-521
+                in_linesize = vc_linesize64(d->width, v210);
         }
         const int groups_mid = (d->width + 5) / 6, groups_last = d->width / 6;  // :89-92
         cudaStream_t s = (cudaStream_t) stream;

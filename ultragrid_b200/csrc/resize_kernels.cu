@@ -41,6 +41,7 @@
 #include <vector>
 
 #include "../../include/ugb200.h"
+#include "filter_args.h"
 #include "host/resize_tables.h"
 #include "host/video_codec.h"
 
@@ -475,21 +476,6 @@ static int layout_of(codec_t c)
         }
 }
 
-// the input frame's bytes: tight rows (resize.c's vc_get_linesize), I420 as its three planes
-static size_t frame_bytes(codec_t c, int w, int h)
-{
-        if (c == I420) {
-                return (size_t) w * h + 2 * (size_t) ((w + 1) / 2) * ((h + 1) / 2);
-        }
-        return (size_t) vc_get_linesize(w, c) * h;
-}
-
-static bool overlap(const void *a, size_t na, const void *b, size_t nb)
-{
-        const uintptr_t x = (uintptr_t) a, y = (uintptr_t) b;
-        return na && nb && x < y + nb && y < x + na;
-}
-
 // what reconfigure_if_needed and resize_frame decide for one input descriptor
 struct Geometry {
         int out[8];  // route, out codec, out_w, out_h, rect x, y, w, h
@@ -729,7 +715,7 @@ static int reconfigure(ResizeState *r, int codec, int width, int height, const G
                         return -2;
                 }
         }
-        const size_t stage = g.out[0] == codec ? 0 : frame_bytes((codec_t) g.out[0], width, height) + kStageSlack;
+        const size_t stage = g.out[0] == codec ? 0 : vc_get_datalen(width, height, (codec_t) g.out[0]) + kStageSlack;
         if (stage != r->stage_bytes) {
                 cudaFree(r->stage);
                 r->stage = nullptr;
@@ -758,7 +744,7 @@ extern "C" UGB_API int ugb200_cf_resize(ugb200_cf_resize_t r, int codec, int wid
         const codec_t route = (codec_t) g.out[0];
         const int ow = g.out[2], oh = g.out[3];
         const long out_ls = vc_get_linesize(ow, (codec_t) g.out[1]);
-        if (overlap(src, frame_bytes((codec_t) codec, width, height), dst, (size_t) out_ls * oh)) {
+        if (overlap(src, vc_get_datalen(width, height, (codec_t) codec), dst, (size_t) out_ls * oh)) {
                 return -1;
         }
         const cudaStream_t st = (cudaStream_t) stream;
