@@ -92,8 +92,8 @@ UGB_API int ugb200_jpeg_encode_into_ex(ugb200_jpeg_encoder *enc, const void *src
 
 /* Measurement: with stage timing on, every encode records CUDA events between its kernels on the encoder's stream;
  * ugb200_jpeg_encoder_stage_times waits for the last encode and returns the device time in microseconds of
- * us[0] the DCT + entropy kernel (one-kernel form: the whole fused kernel; split path: the DCT + Huffman pair), us[1] the restart-segment
- * assembly kernel of the two-kernel form (0 otherwise), us[2] the offset scan, us[3] the compaction. */
+ * us[0] the DCT + entropy kernel (fused path: the whole fused kernel; split path: the DCT + Huffman pair), us[1] always 0 (it was the
+ * restart-segment assembly kernel of a retired two-kernel form; the slot keeps the layout), us[2] the offset scan, us[3] the compaction. */
 UGB_API int ugb200_jpeg_encoder_stage_timing(ugb200_jpeg_encoder *enc, int enable);
 UGB_API int ugb200_jpeg_encoder_stage_times(ugb200_jpeg_encoder *enc, float us[4]);
 

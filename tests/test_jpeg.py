@@ -296,28 +296,6 @@ def test_gpu_noise_takes_serial_route_then_adapts(orc, codec, q):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("form", ["1", "8"])
-@pytest.mark.parametrize("codec", [UYVY, RGB])
-def test_gpu_two_kernel_form_is_byte_identical(orc, monkeypatch, codec, form):
-    """UGB200_JPEG_TWO_KERNELS (read when the encoder is created): block kernel writing the bit strings to global memory + assembly kernel.
-    Natural content (fast route), noise (blocks over the cap: coded again from the coefficient dump; then a larger cap), ragged sizes."""
-    import torch
-    from ultragrid_b200 import api
-    monkeypatch.setenv("UGB200_JPEG_TWO_KERNELS", form)
-    enc = api.JpegEncoder()
-    monkeypatch.delenv("UGB200_JPEG_TWO_KERNELS")
-    bpp = 2 if codec == UYVY else 3
-    for w, h, q in ((1920, 1080, 90), (320, 96, 100), (322, 50, 75)):
-        rgb = natural_rgb(w, h, 5).reshape(-1)
-        nat = rgb if codec == RGB else util.convert_cpu(orc, "orc_convert", RGB, UYVY, rgb, w, h)
-        noise = util.rng_bytes(w * h * bpp, 13)
-        for src in (nat, noise, noise, nat):
-            enc.encode_device(torch.from_numpy(src).cuda(), w, h, codec, quality=q)
-            assert enc.result() == orc_encode(orc, src, w, h, codec, q, 0), (w, h, q)
-    enc.close()
-
-
-@pytest.mark.gpu
 @pytest.mark.parametrize("codec,w,h,pad", [(UYVY, 100, 52, 24), (UYVY, 1920, 64, 64), (RGB, 77, 33, 5), (UYVY, 98, 50, 4)])
 def test_gpu_encoder_honours_the_source_pitch(orc, codec, w, h, pad):
     """rows further apart than one line (device and host input): the same stream as from the tight frame"""

@@ -314,11 +314,9 @@ def test_gpu_two_encoders_on_two_streams(al, orc):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("knob,value", [("UGB200_JPEG_SPLIT", "1"), ("UGB200_JPEG_SINGLE_PASS", "1"), ("UGB200_JPEG_CAP", "12"),
-                                        ("UGB200_JPEG_TWO_KERNELS", "1")])
+@pytest.mark.parametrize("knob,value", [("UGB200_JPEG_SPLIT", "1"), ("UGB200_JPEG_SINGLE_PASS", "1"), ("UGB200_JPEG_CAP", "12")])
 def test_gpu_alternative_routes_give_the_same_bytes(knob, value):
-    """process-wide switches: the byte-exactness tests once more in a child process (the split path takes every RGBA stream there; the
-    two-kernel form falls back to the one-kernel form for RGBA)"""
+    """process-wide switches: the byte-exactness tests once more in a child process (the split path takes every RGBA stream there)"""
     env = dict(os.environ, **{knob: value})
     r = subprocess.run([sys.executable, "-m", "pytest", os.path.abspath(__file__), "-m", "gpu", "-q", "-x", "-k",
                         "equals_oracle_bytes or padded_pitch"], env=env, capture_output=True, text=True, timeout=900)

@@ -646,8 +646,8 @@ def test_gpu_encoder_8k_sampled_segments(orc, pl, name):  # noqa: F811
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("knob,value", [("UGB200_JPEG_SPLIT", "1"), ("UGB200_JPEG_SINGLE_PASS", "1"), ("UGB200_JPEG_TWO_KERNELS", "1"),
-                                        ("UGB200_JPEG_TWO_KERNELS", "8"), ("UGB200_JPEG_CAP", "12"), ("UGB200_JPEG_CAP", "24")])
+@pytest.mark.parametrize("knob,value", [("UGB200_JPEG_SPLIT", "1"), ("UGB200_JPEG_SINGLE_PASS", "1"), ("UGB200_JPEG_CAP", "12"),
+                                        ("UGB200_JPEG_CAP", "24")])
 def test_gpu_encoder_routes_equal_exact_dct(knob, value):
     """the process-wide route switches: the encoder tests once more in a child process with the switch set"""
     env = dict(os.environ, **{knob: value, "UGB200_ROUTE": f"{knob}={value}"})

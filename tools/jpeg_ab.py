@@ -1,13 +1,10 @@
-"""A/B timing of the JPEG encoder's kernel forms at 8K (single stream, two streams, per-stage device times).  The form is chosen by environment
-variables read once per process (UGB200_JPEG_TWO_KERNELS), so each variant runs in a child process.
+"""A/B timing of the JPEG encoder's lean and general fused kernels at 8K (single stream, two streams, per-stage device times).  The kernel is
+chosen by an environment variable read once per process (UGB200_JPEG_LEAN), so each variant runs in a child process.
 usage: python tools/jpeg_ab.py            (parent: runs every variant)"""
 import os, subprocess, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-VARIANTS = [("one kernel (default)", {}), ("two_kernels", {"UGB200_JPEG_TWO_KERNELS": "1"}), ("two_kernels_a8", {"UGB200_JPEG_TWO_KERNELS": "8"})]
-if len(sys.argv) > 1 and sys.argv[1] == "quick":
-    VARIANTS = VARIANTS[:2]
-if len(sys.argv) > 1 and sys.argv[1] == "lean":  # the instantiation without fall-back paths (default where the frame geometry allows) against the general kernel
-    VARIANTS = [("lean kernel (default)", {}), ("general kernel", {"UGB200_JPEG_LEAN": "0"}), ("lean kernel again", {})]
+# the instantiation without fall-back paths (default where the frame geometry allows) against the general kernel
+VARIANTS = [("lean kernel (default)", {}), ("general kernel", {"UGB200_JPEG_LEAN": "0"}), ("lean kernel again", {})]
 
 
 def child():

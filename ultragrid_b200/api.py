@@ -605,7 +605,7 @@ class JpegEncoder:
         _check(_L.ugb200_jpeg_encoder_stage_timing(self._h, 1 if enable else 0), "ugb200_jpeg_encoder_stage_timing")
 
     def stage_times(self):
-        """device microseconds of the last encode: (DCT + entropy kernel, segment assembly kernel, offset scan, compaction)"""
+        """device microseconds of the last encode: (DCT + entropy kernel, 0 (a retired kernel's slot), offset scan, compaction)"""
         us = (ctypes.c_float * 4)()
         _check(_L.ugb200_jpeg_encoder_stage_times(self._h, us), "ugb200_jpeg_encoder_stage_times")
         return tuple(float(x) for x in us)

@@ -641,26 +641,18 @@ __device__ __forceinline__ void mbar_wait(unsigned long long *bar, uint32_t pari
 
 /// MINB = resident CTAs per SM the register allocation aims at: 6 (80 registers) for any cap, 7 (72 registers) when the bit buffers are
 /// capped at 12 words or fewer (28 KB of dynamic shared memory per CTA)
-/// BLOCKS_ONLY (round 2, the two-kernel form): the kernel stops behind the entropy phase.  The bit string of every block goes to global memory
-/// (`gbits`, [CTA][word][128 blocks] - the layout of the shared array, so the stores of a warp are contiguous), its length to `glen`, and
-/// jpeg_assemble_kernel builds the restart segments from them.  What that buys: this kernel has no barrier behind its unequal part (a CTA's chroma
-/// warps finish their entropy coding long before its luma warps), needs 16 KB of
-/// shared memory instead of 28, and the assembly runs as a light kernel of its own at full occupancy.  A block longer than `cap` words (noise) also
-/// leaves its coefficients in `gcoef` (DC slot = the DC DIFFERENCE), from which the assembly kernel codes it again inside a serial segment.
 /// LEAN (state j): an instantiation for frames in which EVERY CTA's tile is whole and goes through the copy engine (the host checks the geometry: 8K and other sizes whose
 /// MCU rows are multiples of the tile) - the global-memory fall-back loads, the cp.async staging and the edge handling are not compiled in: about a fifth less code in
 /// a kernel whose instruction fetch shows up in the stall list (`no_instruction`).  Same arithmetic, same bytes.
-template <int FMT, int MINB, bool BLOCKS_ONLY = false, bool LEAN = false>
+template <int FMT, int MINB, bool LEAN = false>
 __global__ void __launch_bounds__(128, MINB) jpeg_fused_kernel(const uint8_t *__restrict__ src, long pitch, jpeg_geom g, uint8_t *__restrict__ slots,
                                                          uint32_t *__restrict__ sizes, uint32_t *__restrict__ local_off,
                                                          uint32_t *__restrict__ cta_total, bool vec_ok, int cap, uint32_t *__restrict__ stats,
-                                                         jpeg_lookback lb, const __grid_constant__ jpeg_qtab qt, const uint32_t *__restrict__ huff,
-                                                         uint32_t *__restrict__ gbits = nullptr, uint16_t *__restrict__ glen = nullptr,
-                                                         int16_t *__restrict__ gcoef = nullptr)
+                                                         jpeg_lookback lb, const __grid_constant__ jpeg_qtab qt, const uint32_t *__restrict__ huff)
 {
         extern __shared__ __align__(128) uint32_t smem[];
         uint32_t *s_coef = smem;                // [32][128] zig-zag coefficients, two int16 per word
-        uint32_t *s_bits = s_coef + 32 * 128;   // [cap][128]   (BLOCKS_ONLY: not allocated - the bit strings live in gbits)
+        uint32_t *s_bits = s_coef + 32 * 128;   // [cap][128]
         uint32_t *s_seg = s_bits + cap * 128;   // [segments of the CTA][bps * cap]
         __shared__ __align__(16) uint32_t s_huff[32 + 512];  // jpeg_hufftab as it lies in global memory: dc[2][16], ac[2][256]
         uint32_t(*const s_dctab)[16] = (uint32_t(*)[16]) s_huff;
@@ -693,7 +685,7 @@ __global__ void __launch_bounds__(128, MINB) jpeg_fused_kernel(const uint8_t *__
                 const int fm = cta_x * 32, mx0 = fm % g.bw, my0 = fm / g.bw;
                 early_tile = LEAN || (vec_ok && cap >= 8 && mx0 + 32 <= g.bw && (mx0 + 32) * 16 <= g.w && (my0 + 1) * 8 <= g.h);
                 if (early_tile && tid == 0) {
-                        uint8_t *tile0 = (uint8_t *) (BLOCKS_ONLY ? s_coef : s_bits);
+                        uint8_t *tile0 = (uint8_t *) s_bits;
                         const uint8_t *gsrc = src + (long) (my0 * 8) * pitch + (long) mx0 * 32;
                         mbar_init(&s_bar, 1);
                         mbar_expect_tx(&s_bar, 8 * 1024 + (uint32_t) sizeof s_huff);
@@ -754,7 +746,7 @@ __global__ void __launch_bounds__(128, MINB) jpeg_fused_kernel(const uint8_t *__
         //         luma and chroma warps read every byte from there instead of fetching it twice.  The tile borrows s_bits and, for a cap below 16
         //         words, the start of s_seg behind it (both are free until phase 2; s_seg is cleared after the DCT).
         bool staged = false;
-        const uint8_t *tile = FMT == FMT_UYVY_422 && !BLOCKS_ONLY ? (const uint8_t *) s_bits : (const uint8_t *) s_coef;
+        const uint8_t *tile = FMT == FMT_UYVY_422 ? (const uint8_t *) s_bits : (const uint8_t *) s_coef;
         if (FMT == FMT_RGB_444) {
                 // The CTA's 128 blocks are consecutive in raster order of ONE component: 8 rows x 3072 bytes of packed RGB (the run may wrap into the
                 // next block row; the tile keeps block order, not image order).  cp.async in 8-byte pieces - a block starts at a multiple of 24 bytes -
@@ -844,7 +836,7 @@ __global__ void __launch_bounds__(128, MINB) jpeg_fused_kernel(const uint8_t *__
         constexpr int zz[64] = { 0,  1,  8,  16, 9,  2,  3,  10, 17, 24, 32, 25, 18, 11, 4,  5,  12, 19, 26, 33, 40, 48,
                                  41, 34, 27, 20, 13, 6,  7,  14, 21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23,
                                  30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53, 60, 61, 54, 47, 55, 62, 63 };
-        if ((FMT == FMT_RGB_444 || BLOCKS_ONLY) && staged) {
+        if (FMT == FMT_RGB_444 && staged) {
                 __syncthreads();  // the tile lies over the coefficient array: every thread has its samples in registers before the first store
         }
         // word k of the block = zig-zag coefficients k (low half) and k + 32 (high half): the non-zero flags of 16 words then add up
@@ -875,13 +867,9 @@ __global__ void __launch_bounds__(128, MINB) jpeg_fused_kernel(const uint8_t *__
         nz &= ~1ull;
         s_dc[pc] = dcv;
         __syncthreads();
-        if (!BLOCKS_ONLY) {
-                for (int i = tid; i < cap * 128; i += 128) {  // the segment images start empty (the input tile, dead by now, may have reached into them)
-                        s_seg[i] = 0;
-                }
+        for (int i = tid; i < cap * 128; i += 128) {  // the segment images start empty (the input tile, dead by now, may have reached into them)
+                s_seg[i] = 0;
         }
-        // linear index of this CTA (the order of cta_total / gbits / glen) and of my block in the frame's scan order
-        const int cta_lin = FMT == FMT_UYVY_422 ? cta_x : cta_y * lb.ctas_per_scan + cta_x;
         // ---- 2. entropy-code my block --------------------------------------------------------------------------------------------
         uint32_t bits = 0;
         if (valid) {
@@ -894,7 +882,7 @@ __global__ void __launch_bounds__(128, MINB) jpeg_fused_kernel(const uint8_t *__
                 } else {
                         pred = (p % bps) == 0 ? 0 : s_dc[blk_col(p - 1)];
                 }
-                block_bits bw = { (BLOCKS_ONLY ? gbits + (size_t) cta_lin * cap * 128 : s_bits) + pc, 0, 0, 0, cap };
+                block_bits bw = { s_bits + pc, 0, 0, 0, cap };
                 const int diff = dcv - pred;
                 int sz = category(diff);
                 bw.put(s_dctab[t][sz] & 0xffff, s_dctab[t][sz] >> 16);
@@ -929,34 +917,6 @@ __global__ void __launch_bounds__(128, MINB) jpeg_fused_kernel(const uint8_t *__
                         bw.put(act[0] & 0xffff, act[0] >> 16);  // EOB
                 }
                 bits = bw.finish();
-                if (BLOCKS_ONLY && bits > (uint32_t) cap * 32u) {
-                        // longer than the cap: the assembly kernel codes this block again from its coefficients (natural order of the split path's
-                        // coefficient buffer: 64 int16 per block in scan order); slot 0 carries the DC difference - the predictor is not known there
-                        const long blk = FMT == FMT_UYVY_422 ? (long) first_mcu * 4 + p : (long) cta_y * g.mcu_per_scan + first_mcu + p;
-                        uint32_t *dst = (uint32_t *) (gcoef + blk * 64);
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) {
-                                const uint32_t w0 = cw[(2 * j) * 128], w1 = cw[(2 * j + 1) * 128];
-                                dst[j] = __byte_perm(w0, w1, 0x5410);       // coefficients 2j, 2j + 1
-                                dst[16 + j] = __byte_perm(w0, w1, 0x7632);  // coefficients 32 + 2j, 33 + 2j
-                        }
-                        ((int16_t *) dst)[0] = (int16_t) diff;
-                }
-        }
-        if (BLOCKS_ONLY) {
-                glen[(size_t) cta_lin * 128 + pc] = (uint16_t) bits;
-                uint32_t mx = bits;
-#pragma unroll
-                for (int d = 16; d > 0; d >>= 1) {
-                        mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, d));
-                }
-                if ((tid & 31) == 0) {
-                        atomicMax(stats, mx);
-                        if (mx > (uint32_t) cap * 32u) {
-                                atomicAdd(stats + 1, 1u);
-                        }
-                }
-                return;
         }
         s_len[pc] = bits;
         const bool overflow = __syncthreads_or(bits > (uint32_t) cap * 32u) != 0;
@@ -1186,171 +1146,6 @@ __global__ void __launch_bounds__(128, MINB) jpeg_fused_kernel(const uint8_t *__
                         }
                         *lb.total = (uint32_t) (end + 2);
                 }
-        }
-}
-
-// ---- restart-segment assembly of the two-kernel form --------------------------------------------------------------------------------------------
-/// Second kernel behind jpeg_fused_kernel<.., BLOCKS_ONLY>: thread t of a CTA owns scan-order block t of the CTA's 128 (same CTA numbering), the
-/// threads of a restart segment sit in one warp.  Phases 3-5 of the one-kernel form: prefix of the bit lengths, the bit strings ORed into the
-/// segment image, byte stuffing, slot + size, CTA prefix of the sizes - with warp-level synchronisation only (a segment never leaves its warp), 12 KB
-/// of shared memory at the default cap and ~40 registers, i.e. at full occupancy.  A segment with a block beyond the cap is coded by its first
-/// thread alone: stored bit strings are appended as they are, the long block is coded again from its coefficients in `gcoef`.
-template <int FMT>
-__global__ void __launch_bounds__(128) jpeg_assemble_kernel(jpeg_geom g, const uint32_t *__restrict__ gbits, const uint16_t *__restrict__ glen,
-                                                            const int16_t *__restrict__ gcoef, uint8_t *__restrict__ slots, uint32_t *__restrict__ sizes,
-                                                            uint32_t *__restrict__ local_off, uint32_t *__restrict__ cta_total, int cap, int ctas_per_scan,
-                                                            const uint32_t *__restrict__ huff)
-{
-        extern __shared__ __align__(128) uint32_t smem[];
-        uint32_t *s_seg = smem;                 // [segments of the CTA][bps * cap]
-        uint32_t *s_stage = smem + cap * 128;   // stuffing area, same partition
-        __shared__ uint32_t s_warp[4];
-        const int tid = threadIdx.x;
-        asm volatile("griddepcontrol.launch_dependents;");
-        const int cta_x = FMT == FMT_UYVY_422 ? blockIdx.x : blockIdx.x % ctas_per_scan, cta_y = FMT == FMT_UYVY_422 ? 0 : blockIdx.x / ctas_per_scan;
-        const int cta_lin = blockIdx.x;  // = cta_y * ctas_per_scan + cta_x
-        const int bps = g.ri * g.blocks_per_mcu;
-        const int first_mcu = cta_x * (FMT == FMT_UYVY_422 ? 32 : 128);
-        for (int i = tid & 31; i < 32 * cap; i += 32) {  // every warp clears the images of its own segments
-                s_seg[(tid >> 5) * 32 * cap + i] = 0;
-        }
-        __syncwarp();
-        asm volatile("griddepcontrol.wait;" ::: "memory");  // bit strings and lengths of the kernel in front (programmatic dependent launch)
-        const int sg = tid / bps, gl = tid % bps;
-        const unsigned lane32 = tid & 31;
-        const int ls = first_mcu / g.ri + sg;
-        const int seg_global = FMT == FMT_UYVY_422 ? ls : cta_y * g.seg_per_scan + ls;
-        const bool seg_valid = ls < g.seg_per_scan && (long) ls * g.ri < g.mcu_per_scan;
-        const unsigned gmask = bps == 32 ? 0xffffffffu : (((1u << bps) - 1u) << (lane32 - gl));
-        const int tc = blk_col(tid);
-        const uint32_t L = glen[(size_t) cta_lin * 128 + tc];
-        const uint32_t *myb = gbits + (size_t) cta_lin * cap * 128 + tc;
-        const bool seg_over = (__ballot_sync(0xffffffffu, L > (uint32_t) cap * 32u) & gmask) != 0;
-        uint32_t written = 0;
-        if (seg_over) {
-                if (gl == 0 && seg_valid) {  // serial: the segment's first thread appends the 16 strings one after the other
-                        uint32_t *base = (uint32_t *) (slots + (long) seg_global * g.slot);
-                        bit_writer bw = { base, 0, 0, 0, 0 };
-                        for (int q = tid; q < tid + bps; ++q) {
-                                const int m = first_mcu + (FMT == FMT_UYVY_422 ? q >> 2 : q);
-                                if (m >= g.mcu_per_scan) {
-                                        break;
-                                }
-                                const int qc = blk_col(q);
-                                const uint32_t Lq = glen[(size_t) cta_lin * 128 + qc];
-                                if (Lq <= (uint32_t) cap * 32u) {
-                                        const uint32_t *qb = gbits + (size_t) cta_lin * cap * 128 + qc;
-                                        for (uint32_t w = 0; w * 32 < Lq; ++w) {
-                                                const uint32_t v = qb[w * 128];
-                                                const int n = (int) min(32u, Lq - w * 32), first = min(n, 16);  // the top n bits of v, MSB first
-                                                bw.put(v >> (32 - first), first);
-                                                if (n > 16) {
-                                                        bw.put(v >> (32 - n), n - 16);  // put() keeps the low n - 16 bits
-                                                }
-                                        }
-                                        continue;
-                                }
-                                // the block's own coefficients (natural order; slot 0 = DC difference)
-                                const int comp = FMT == FMT_UYVY_422 ? ((q & 3) < 2 ? 0 : (q & 3) - 1) : cta_y;
-                                const int t = comp == 0 ? 0 : 1;
-                                const long blk = FMT == FMT_UYVY_422 ? (long) first_mcu * 4 + q : (long) cta_y * g.mcu_per_scan + first_mcu + q;
-                                const int16_t *zz = gcoef + blk * 64;
-                                const uint32_t *dct = huff + 16 * t, *act = huff + 32 + 256 * t;
-                                const int diff = zz[0];
-                                int sz = category(diff);
-                                bw.put(dct[sz] & 0xffff, dct[sz] >> 16);
-                                if (sz) {
-                                        bw.put((uint32_t) (diff < 0 ? diff - 1 : diff), sz);
-                                }
-                                int prev = 0;
-                                for (int i = 1; i < 64; ++i) {
-                                        const int v = zz[i];
-                                        if (v == 0) {
-                                                continue;
-                                        }
-                                        int run = i - prev - 1;
-                                        prev = i;
-                                        while (run > 15) {
-                                                bw.put(act[0xF0] & 0xffff, act[0xF0] >> 16);
-                                                run -= 16;
-                                        }
-                                        sz = category(v);
-                                        const uint32_t e = act[(run << 4) | sz];
-                                        bw.put(((e & 0xffff) << sz) | ((uint32_t) (v < 0 ? v - 1 : v) & ((1u << sz) - 1u)), (int) (e >> 16) + sz);
-                                }
-                                if (prev != 63) {
-                                        bw.put(act[0] & 0xffff, act[0] >> 16);
-                                }
-                        }
-                        bw.flush_bits();
-                        if (ls != g.seg_per_scan - 1) {
-                                bw.emit_byte(0xFF);
-                                bw.emit_byte(0xD0 + (ls & 7));
-                        }
-                        written = bw.finish(base);
-                        sizes[seg_global] = written;
-                }
-        } else {
-                uint32_t incl = L;
-                for (int d = 1; d < bps; d <<= 1) {
-                        const uint32_t o = __shfl_up_sync(gmask, incl, d, bps);
-                        if (gl >= d) {
-                                incl += o;
-                        }
-                }
-                const uint32_t T = __shfl_sync(gmask, incl, bps - 1, bps);
-                uint32_t *seg = s_seg + sg * bps * cap;
-                {
-                        const uint32_t off = incl - L, sh = off & 31;
-                        uint32_t *d = seg + (off >> 5);
-                        for (uint32_t w = 0; w * 32 < L; ++w) {
-                                const uint32_t v = myb[w * 128];
-                                atomicOr(d + w, v >> sh);
-                                if (sh && (v << (32 - sh))) {
-                                        atomicOr(d + w + 1, v << (32 - sh));
-                                }
-                        }
-                        if (gl == 0 && (T & 7)) {  // pad the last byte with ones (T.81 F.1.2.3)
-                                const uint32_t pad = 8 - (T & 7);
-                                atomicOr(seg + (T >> 5), ((1u << pad) - 1u) << (32 - (T & 31) - pad));
-                        }
-                }
-                __syncwarp(gmask);
-                if (seg_valid) {
-                        const int rst = ls != g.seg_per_scan - 1 ? 0xD0 + (ls & 7) : -1;
-                        uint8_t *slot = slots + (long) seg_global * g.slot;
-                        written = stuff_segment_words(slot, (uint8_t *) s_stage + (size_t) sg * bps * cap * 4, (uint32_t) (bps * cap * 4), seg, T, bps, gl, gmask, rst);
-                        if (written == 0xFFFFFFFFu) {
-                                written = stuff_segment(slot, seg, T, bps, gl, lane32, gmask, rst);
-                        }
-                        if (gl == 0) {
-                                sizes[seg_global] = written;
-                        }
-                }
-        }
-        // CTA prefix of the segment sizes (first level of the stream-offset scan, as in the one-kernel form)
-        const uint32_t mine = (gl == 0 && seg_valid) ? written : 0;
-        uint32_t inc2 = mine;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-                const uint32_t o = __shfl_up_sync(0xffffffffu, inc2, d);
-                if (lane32 >= (unsigned) d) {
-                        inc2 += o;
-                }
-        }
-        if (lane32 == 31) {
-                s_warp[tid >> 5] = inc2;
-        }
-        __syncthreads();
-        uint32_t before = 0;
-        for (int w = 0; w < (tid >> 5); ++w) {
-                before += s_warp[w];
-        }
-        if (gl == 0 && seg_valid) {
-                local_off[seg_global] = before + inc2 - mine;
-        }
-        if (tid == 127) {
-                cta_total[cta_lin] = before + inc2;
         }
 }
 
@@ -1686,9 +1481,6 @@ struct ugb200_jpeg_encoder {
         uint32_t *d_huff = nullptr;      // jpeg_hufftab on the device
         unsigned long long *lb_state = nullptr;  // look-back state of the single-pass compaction ([0] = ticket counter)
         size_t lb_cap = 0;
-        uint32_t *gbits = nullptr;               // two-kernel form: bit strings [CTA][cap][128] and lengths [CTA][128] of all blocks
-        uint16_t *glen = nullptr;
-        size_t gbits_cap = 0, glen_cap = 0;
         size_t coef_cap = 0, slots_cap = 0, out_cap = 0, seg_cap = 0, staging_cap = 0, cta_cap = 0;
         // pinned host buffers
         uint8_t *h_out = nullptr, *h_in = nullptr;
@@ -1701,10 +1493,9 @@ struct ugb200_jpeg_encoder {
         bool last_vec_ok = false, last_fused = false;
         cudaEvent_t stats_ev = nullptr;  // recorded behind the copy of h_total: lets an asynchronous caller adapt the cap too
         bool stats_pending = false;
-        int form = 0;  // 0: one fused kernel (default), 1 / 2: block kernel + assembly kernel
-        bool attr_set[4] = { false, false, false, false };  // cudaFuncSetAttribute done for the fused UYVY / RGB, assembly, fused RGBA kernels on this encoder's device
+        bool attr_set[3] = { false, false, false };  // cudaFuncSetAttribute done for the fused UYVY / RGB / RGBA kernel on this encoder's device
         bool stage_timing = false;       // ugb200_jpeg_encoder_stage_timing: events between the kernels of an encode
-        cudaEvent_t stage_ev[5] = { nullptr, nullptr, nullptr, nullptr, nullptr };
+        cudaEvent_t stage_ev[4] = { nullptr, nullptr, nullptr, nullptr };  // in front of the DCT + entropy kernel(s), behind them, behind the scan, behind the compaction
 };
 
 namespace {
@@ -1957,8 +1748,6 @@ ugb200_jpeg_encoder *ugb200_jpeg_encoder_create(cuda_wrapper_stream_t stream)
         ugb200_jpeg_encoder *e = new (std::nothrow) ugb200_jpeg_encoder;
         if (e) {
                 e->stream = (cudaStream_t) stream;
-                const char *f = getenv("UGB200_JPEG_TWO_KERNELS");  // "1": two-kernel form, "8": the same with the 64-register block kernel
-                e->form = !f ? 0 : f[0] == '8' ? 2 : 1;
         }
         return e;
 }
@@ -1971,7 +1760,7 @@ void ugb200_jpeg_encoder_destroy(ugb200_jpeg_encoder *e)
         cudaStreamSynchronize(e->stream);
         cudaFree(e->coef), cudaFree(e->slots), cudaFree(e->out), cudaFree(e->staging);
         cudaFree(e->sizes), cudaFree(e->offsets), cudaFree(e->cta_total), cudaFree(e->total), cudaFree(e->lb_state), cudaFree(e->d_huff);
-        cudaFree(e->gbits), cudaFree(e->glen), cudaFree(e->planes);
+        cudaFree(e->planes);
         cudaFreeHost(e->h_out), cudaFreeHost(e->h_in), cudaFreeHost(e->h_total);
         if (e->stats_ev) {
                 cudaEventDestroy(e->stats_ev);
@@ -1994,7 +1783,7 @@ static void adapt_cap(ugb200_jpeg_encoder *e)
         e->stats_pending = false;
 }
 
-static int launch_tail(ugb200_jpeg_encoder *e, int nctas, int segs_per_cta, int ctas_per_scan, bool single_pass, bool two_kernels);
+static int launch_tail(ugb200_jpeg_encoder *e, int nctas, int segs_per_cta, int ctas_per_scan, bool single_pass);
 
 /// the packed layouts: UYVY 4:2:2, RGB 4:4:4 (ugb200_jpeg_encode_device) and RGBA 4:4:4:4 (ugb200_jpeg_encode_device_ex only)
 static int encode_packed(ugb200_jpeg_encoder *e, const void *src, long pitch, int width, int height, int fmt, const struct ugb200_jpeg_params *params)
@@ -2018,7 +1807,7 @@ static int encode_packed(ugb200_jpeg_encoder *e, const void *src, long pitch, in
         const bool fused = !force_split && !g.interleaved && (bps == 4 || bps == 8 || bps == 16 || bps == 32);
         e->last_fused = fused;
         int nctas, segs_per_cta, ctas_per_scan;
-        bool single_pass = false, two_kernels = false;
+        bool single_pass = false;
         if (e->stage_timing) {
                 cudaEventRecord(e->stage_ev[0], e->stream);
         }
@@ -2045,7 +1834,7 @@ static int encode_packed(ugb200_jpeg_encoder *e, const void *src, long pitch, in
                 }
                 const bool seven = cap <= 12;  // 28 KB per CTA: seven CTAs (28 warps) fit an SM
                 const int max_smem = (int) ((32 * 128 + 2 * kBlkWords * 128) * sizeof(uint32_t));
-                const int attr = fmt == FMT_UYVY_422 ? 0 : fmt == FMT_RGB_444 ? 1 : 3;
+                const int attr = fmt == FMT_UYVY_422 ? 0 : fmt == FMT_RGB_444 ? 1 : 2;
                 if (!e->attr_set[attr]) {  // per encoder = per device context: the attribute does not carry over to another GPU
                         if (fmt == FMT_UYVY_422) {
                                 cudaFuncSetAttribute(jpeg_fused_kernel<FMT_UYVY_422, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem);
@@ -2057,57 +1846,9 @@ static int encode_packed(ugb200_jpeg_encoder *e, const void *src, long pitch, in
                         e->attr_set[attr] = true;
                 }
                 const dim3 grid(nctas);  // RGB: component fastest (two-pass) or tickets running over the three scans (single pass)
-                // two-kernel form (UGB200_JPEG_TWO_KERNELS at encoder creation): blocks -> bit strings in global memory, then the segment assembly as a
-                // kernel of its own.  Not the default: on an earlier GPU it was no faster on one stream and only slightly faster with two encoders alternating.
-                const bool eight = e->form == 2;  // 64 registers / 8 CTAs per SM for the block kernel
-                two_kernels = !single_pass && e->form != 0 && fmt != FMT_RGBA_4444;  // RGBA: the one-kernel form only
-                if (two_kernels) {
-                        if (!grow(e->gbits, e->gbits_cap, (size_t) nctas * cap * 128) || !grow(e->glen, e->glen_cap, (size_t) nctas * 128)) {
-                                return -2;
-                        }
-                        const size_t smem_a = fmt == FMT_UYVY_422 ? 32 * 128 * 4 : 8 * 3072;  // the coefficient array; the RGB tile over it is 24 KB
-#define UGB_BLOCKS(FMT, MINB)                                                                                                                                  \
-        jpeg_fused_kernel<FMT, MINB, true><<<grid, 128, smem_a, e->stream>>>((const uint8_t *) src, pitch, g, e->slots, e->sizes, e->offsets, e->cta_total, vec_ok, \
-                                                                             cap, e->total + 1, lb, e->qt, e->d_huff, e->gbits, e->glen, e->coef)
-                        if (fmt == FMT_UYVY_422) {
-                                if (eight) {
-                                        UGB_BLOCKS(FMT_UYVY_422, 8);
-                                } else {
-                                        UGB_BLOCKS(FMT_UYVY_422, 7);
-                                }
-                        } else {
-                                if (eight) {
-                                        UGB_BLOCKS(FMT_RGB_444, 8);
-                                } else {
-                                        UGB_BLOCKS(FMT_RGB_444, 7);
-                                }
-                        }
-#undef UGB_BLOCKS
-                        if (e->stage_timing) {
-                                cudaEventRecord(e->stage_ev[1], e->stream);
-                        }
-                        cudaLaunchAttribute pdl[1];
-                        pdl[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-                        pdl[0].val.programmaticStreamSerializationAllowed = 1;
-                        cudaLaunchConfig_t cfg{};
-                        cfg.stream = e->stream, cfg.attrs = pdl, cfg.numAttrs = e->stage_timing ? 0 : 1;
-                        cfg.gridDim = dim3((unsigned) nctas), cfg.blockDim = dim3(128), cfg.dynamicSmemBytes = (size_t) cap * 1024;
-                        if (cfg.dynamicSmemBytes > 48 * 1024 && !e->attr_set[2]) {
-                                cudaFuncSetAttribute(jpeg_assemble_kernel<FMT_UYVY_422>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlkWords * 1024);
-                                cudaFuncSetAttribute(jpeg_assemble_kernel<FMT_RGB_444>, cudaFuncAttributeMaxDynamicSharedMemorySize, kBlkWords * 1024);
-                                e->attr_set[2] = true;
-                        }
-                        if (fmt == FMT_UYVY_422) {
-                                cudaLaunchKernelEx(&cfg, jpeg_assemble_kernel<FMT_UYVY_422>, g, (const uint32_t *) e->gbits, (const uint16_t *) e->glen, (const int16_t *) e->coef,
-                                                   e->slots, e->sizes, e->offsets, e->cta_total, cap, ctas_per_scan, (const uint32_t *) e->d_huff);
-                        } else {
-                                cudaLaunchKernelEx(&cfg, jpeg_assemble_kernel<FMT_RGB_444>, g, (const uint32_t *) e->gbits, (const uint16_t *) e->glen, (const int16_t *) e->coef,
-                                                   e->slots, e->sizes, e->offsets, e->cta_total, cap, ctas_per_scan, (const uint32_t *) e->d_huff);
-                        }
-                } else {
 #define UGB_FUSED(FMT, MINB, LEAN)                                                                                                                        \
-        jpeg_fused_kernel<FMT, MINB, false, LEAN><<<grid, 128, smem, e->stream>>>((const uint8_t *) src, pitch, g, e->slots, e->sizes, e->offsets, e->cta_total, vec_ok, \
-                                                                                  cap, e->total + 1, lb, e->qt, e->d_huff)
+        jpeg_fused_kernel<FMT, MINB, LEAN><<<grid, 128, smem, e->stream>>>((const uint8_t *) src, pitch, g, e->slots, e->sizes, e->offsets, e->cta_total, vec_ok, \
+                                                                           cap, e->total + 1, lb, e->qt, e->d_huff)
                 // every CTA's tile whole and bulk-copyable?  (the conditions of the kernel's `early_tile`, for all CTAs at once; UGB200_JPEG_LEAN=0 keeps the general kernel)
                 static const bool allow_lean = getenv("UGB200_JPEG_LEAN") == nullptr || atoi(getenv("UGB200_JPEG_LEAN")) != 0;
                 const bool lean = allow_lean && vec_ok && cap >= 8 && (g.h & 7) == 0 &&
@@ -2129,7 +1870,6 @@ static int encode_packed(ugb200_jpeg_encoder *e, const void *src, long pitch, in
                         }
                 }
 #undef UGB_FUSED
-                }
         } else {  // split path: any restart interval
                 const int dct_ctas = fmt == FMT_UYVY_422 ? (g.mcu_per_scan + 31) / 32 : (g.nblocks + 127) / 128;
                 nctas = (g.nseg + 127) / 128, segs_per_cta = 128, ctas_per_scan = 0;
@@ -2141,7 +1881,7 @@ static int encode_packed(ugb200_jpeg_encoder *e, const void *src, long pitch, in
                         jpeg_huffman_kernel<false><<<nctas, 128, 0, e->stream>>>(e->coef, g, e->slots, e->sizes, e->offsets, e->cta_total, e->d_huff, e->lay);
                 }
         }
-        return launch_tail(e, nctas, segs_per_cta, ctas_per_scan, single_pass, two_kernels);
+        return launch_tail(e, nctas, segs_per_cta, ctas_per_scan, single_pass);
 }
 
 int ugb200_jpeg_encode_device(ugb200_jpeg_encoder *e, const void *src, long pitch, int width, int height, int codec,
@@ -2157,14 +1897,11 @@ int ugb200_jpeg_encode_device(ugb200_jpeg_encoder *e, const void *src, long pitc
 }
 
 /// the common end of an encode: offset scan + compaction (nothing behind the single-pass form), the copy of the stream size and statistics
-static int launch_tail(ugb200_jpeg_encoder *e, int nctas, int segs_per_cta, int ctas_per_scan, bool single_pass, bool two_kernels)
+static int launch_tail(ugb200_jpeg_encoder *e, int nctas, int segs_per_cta, int ctas_per_scan, bool single_pass)
 {
         const jpeg_geom &g = e->g;
         if (e->stage_timing) {
-                if (!two_kernels) {
-                        cudaEventRecord(e->stage_ev[1], e->stream);
-                }
-                cudaEventRecord(e->stage_ev[2], e->stream);  // behind the assembly kernel (= behind the one-kernel form when there is none)
+                cudaEventRecord(e->stage_ev[1], e->stream);
         }
         if (!single_pass) {
                 // programmatic dependent launch: the scan and the compaction are set up while their predecessor drains (they wait for its results
@@ -2179,7 +1916,7 @@ static int launch_tail(ugb200_jpeg_encoder *e, int nctas, int segs_per_cta, int 
                 cfg.gridDim = dim3(1), cfg.blockDim = dim3(1024);
                 cudaLaunchKernelEx(&cfg, jpeg_scan_kernel, e->cta_total, nctas, g, e->total, e->lay.nscans);
                 if (e->stage_timing) {
-                        cudaEventRecord(e->stage_ev[3], e->stream);
+                        cudaEventRecord(e->stage_ev[2], e->stream);
                 }
                 cfg.gridDim = dim3((unsigned) (((long) g.nseg * kCompactLanes + 255) / 256)), cfg.blockDim = dim3(256);
                 cudaLaunchKernelEx(&cfg, jpeg_compact_kernel, (const uint8_t *) e->slots, (const uint32_t *) e->sizes, (const uint32_t *) e->offsets,
@@ -2187,9 +1924,9 @@ static int launch_tail(ugb200_jpeg_encoder *e, int nctas, int segs_per_cta, int 
         }
         if (e->stage_timing) {
                 if (single_pass) {
-                        cudaEventRecord(e->stage_ev[3], e->stream);
+                        cudaEventRecord(e->stage_ev[2], e->stream);
                 }
-                cudaEventRecord(e->stage_ev[4], e->stream);
+                cudaEventRecord(e->stage_ev[3], e->stream);
         }
         if (cudaGetLastError() != cudaSuccess) {
                 return -2;
@@ -2298,7 +2035,7 @@ static int encode_planar(ugb200_jpeg_encoder *e, const void *src, long pitch, in
         jpeg_dct_kernel<true><<<(g.nblocks + 127) / 128, 128, 0, e->stream>>>(nullptr, 0, g, e->coef, vec_ok, e->qt, L);
         const int nctas = (g.nseg + 127) / 128;
         jpeg_huffman_kernel<true><<<nctas, 128, 0, e->stream>>>(e->coef, g, e->slots, e->sizes, e->offsets, e->cta_total, e->d_huff, L);
-        return launch_tail(e, nctas, 128, 0, false, false);
+        return launch_tail(e, nctas, 128, 0, false);
 }
 
 int ugb200_jpeg_encode_device_ex(ugb200_jpeg_encoder *e, const void *src, long pitch, int width, int height, int codec,
@@ -2342,16 +2079,16 @@ int ugb200_jpeg_encoder_stage_times(ugb200_jpeg_encoder *e, float us[4])
         if (!e || !us || !e->stage_timing || !e->pending) {
                 return -1;
         }
-        if (cudaEventSynchronize(e->stage_ev[4]) != cudaSuccess) {
+        if (cudaEventSynchronize(e->stage_ev[3]) != cudaSuccess) {
                 return -2;
         }
-        for (int i = 0; i < 4; ++i) {
-                float ms = 0;
-                if (cudaEventElapsedTime(&ms, e->stage_ev[i], e->stage_ev[i + 1]) != cudaSuccess) {
+        float ms[3];
+        for (int i = 0; i < 3; ++i) {
+                if (cudaEventElapsedTime(&ms[i], e->stage_ev[i], e->stage_ev[i + 1]) != cudaSuccess) {
                         return -2;
                 }
-                us[i] = ms * 1000.0f;
         }
+        us[0] = ms[0] * 1000.0f, us[1] = 0, us[2] = ms[1] * 1000.0f, us[3] = ms[2] * 1000.0f;
         return 0;
 }
 
