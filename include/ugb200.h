@@ -55,6 +55,19 @@ UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *dst, long d
                           int dst_len, int height, long src_size, int rshift, int gshift, int bshift,
                           cuda_wrapper_stream_t stream);
 
+/* Colour space of the RGB <-> YCbCr converters: the values of UltraGrid's enum colorspace (src/color_space.h:129-133).  A binding passes
+ * get_default_cs(), which is UGB_CS_601 under `--param color-601` and UGB_CS_709 otherwise. */
+enum ugb200_colorspace {
+        UGB_CS_DFL = 0,  /* BT.709, UltraGrid's default */
+        UGB_CS_601 = 1,  /* BT.601 */
+        UGB_CS_709 = 2,  /* BT.709 */
+};
+/* ugb200_pixfmt_convert with the Q14 coefficients of `cs` (get_color_coeffs(CS_DFL, depth) of an UltraGrid whose default colour space is `cs`)
+ * in every converter whose reference body reads them; the others give the same bytes for every `cs`.  ugb200_pixfmt_convert is this with
+ * UGB_CS_709.  A `cs` outside enum ugb200_colorspace returns -1 and writes nothing. */
+UGB_API int ugb200_pixfmt_convert_cs(int in_codec, int out_codec, void *dst, long dst_pitch, const void *src, long src_pitch, int dst_len, int height,
+                                     long src_size, int rshift, int gshift, int bshift, int cs, cuda_wrapper_stream_t stream);
+
 /* Launch form of the line converters: -1 (default) = per converter, whichever measured faster at 8K (staged through shared memory with coalesced 16-byte
  * accesses, or one chunk per thread straight from / to global memory); 0 = never staged; 1 / 2 / 3 = input and output / output only / input only staged whenever pointers and pitches are 16-byte aligned.
  * The results are identical; the knob exists for the sweep (tools/pixfmt_sweep.py) and the tests.  Env UGB200_LINE_STAGED sets the initial value.

@@ -49,11 +49,18 @@ UGB_API int ugb200_to_lavc_supported(int in_codec, int av_pixfmt);
  * of 8, UYVY pixel pairs ...), except that no sample is written beyond a plane row's linesize. */
 UGB_API int ugb200_to_lavc_convert(int in_codec, int av_pixfmt, const struct ugb200_av_planes *out, const void *in_data, int width, int height,
                                    cuda_wrapper_stream_t stream);
+/* ugb200_to_lavc_convert with the colour space `cs` (enum ugb200_colorspace, include/ugb200.h): the RGB-family sources (R10k, RG48, R12L, RGB ->
+ * YUV) use the coefficients of get_color_coeffs(CS_DFL, depth) of an UltraGrid whose default colour space is `cs`; the YCbCr sources ignore it.
+ * ugb200_to_lavc_convert is this with UGB_CS_709.  Any other `cs` returns -1 and writes nothing. */
+UGB_API int ugb200_to_lavc_convert_cs(int in_codec, int av_pixfmt, const struct ugb200_av_planes *out, const void *in_data, int width, int height, int cs,
+                                      cuda_wrapper_stream_t stream);
 
 /* The hook shape of to_lavc_vid_conv_cuda.h:60-65.  The state owns device planes of the right size (AVFrame role); `in_data` is a HOST frame
  * (as the reference's hook gets it) unless in_is_device.  Returns the planes (device memory, valid until the next call), NULL on error. */
 struct ugb200_to_lavc_conv;
 UGB_API struct ugb200_to_lavc_conv *ugb200_to_lavc_vid_conv_init(int in_codec, int width, int height, int av_pixfmt);
+/* the same state converting in the colour space `cs` (as ugb200_to_lavc_convert_cs); NULL for a `cs` outside enum ugb200_colorspace */
+UGB_API struct ugb200_to_lavc_conv *ugb200_to_lavc_vid_conv_init_cs(int in_codec, int width, int height, int av_pixfmt, int cs);
 UGB_API const struct ugb200_av_planes *ugb200_to_lavc_vid_conv(struct ugb200_to_lavc_conv *state, const char *in_data, int in_is_device);
 UGB_API void ugb200_to_lavc_vid_conv_destroy(struct ugb200_to_lavc_conv **state);
 

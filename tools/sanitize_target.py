@@ -1,5 +1,5 @@
 """exercises every C-ABI entry point once or twice at small, odd sizes - meant to run under `compute-sanitizer --tool memcheck`"""
-import os, sys
+import ctypes, os, sys
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -17,7 +17,8 @@ for inc, outc in ([] if ONLY in ("jpeg", "staged") else PAIRS):  # line converte
         src = torch.randint(0, 256, (ls_i * h + 64,), dtype=torch.uint8, device="cuda")  # MAX_PADDING of over-read slack, video_codec.h:61
         dst = torch.zeros(ls_o * h + 64, dtype=torch.uint8, device="cuda")
         api.pixfmt_convert(inc, outc, src, w, h, dst=dst)
-        n += 1
+        api.pixfmt_convert(inc, outc, src, w, h, dst=dst, cs=api.CS_601)  # ugb200_pixfmt_convert_cs: the BT.601 instantiations
+        n += 2
 for name, depth in ([] if ONLY in ("jpeg", "staged") else pc.all_cases()):  # planar converters
     for w, h in ((50, 5), (17, 3), (64, 4)):
         if name == "yuv420_to_i420" and (w % 2 or h % 2):
@@ -230,6 +231,12 @@ if ONLY not in ("jpeg", "staged"):
             for _, lss, off in tle.plane_modes(fmt, w, h):
                 assert tle.gpu_to_lavc(L2, torch, inc, fmt, src, w, h, lss, off)[0] == 0
                 n += 1
+            planes = [torch.zeros(ls * rows, dtype=torch.uint8, device="cuda") for ls, rows in api.av_plane_shapes(fmt, w, h)]
+            api.to_lavc(inc, fmt, torch.from_numpy(src).cuda(), w, h, planes=planes, cs=api.CS_601)  # ugb200_to_lavc_convert_cs
+            st = L2.ugb200_to_lavc_vid_conv_init_cs(inc, w, h, tle.AV[fmt], api.CS_601)
+            assert st and L2.ugb200_to_lavc_vid_conv(st, src.ctypes.data, 0)
+            L2.ugb200_to_lavc_vid_conv_destroy(ctypes.byref(ctypes.c_void_p(st)))
+            n += 2
     for fmt, outc in tle.from_lavc_pairs():
         for w, h in ((47, 5), (15, 3)):
             pl = tle.av_planes_in(fmt, w, h, 2, pad=3)

@@ -62,6 +62,16 @@ constexpr color_coeffs compute_color_coeffs(double kr, double kb, int depth)
 constexpr color_coeffs coeffs_709(int depth) { return compute_color_coeffs(KR_709, KB_709, depth); }
 constexpr color_coeffs coeffs_601(int depth) { return compute_color_coeffs(KR_601, KB_601, depth); }
 
+/// The coefficient set of get_color_coeffs(CS_DFL, depth) as a compile-time parameter of the converters that read it: bt709 under UltraGrid's
+/// default, bt601 under `--param color-601` (get_default_cs(), color_space.c:186-191).  A converter takes one as a template argument, so its
+/// coefficients stay immediates in each instantiation; the launcher picks the instantiation from the caller's colour space.
+struct bt709 {
+        static constexpr color_coeffs at(int depth) { return coeffs_709(depth); }
+};
+struct bt601 {
+        static constexpr color_coeffs at(int depth) { return coeffs_601(depth); }
+};
+
 // ---- pinned to the reference build (SURVEY.md 8a A3) --------------------------------------------
 namespace pin {
 constexpr color_coeffs c8 = coeffs_709(8), c10 = coeffs_709(10), c16 = coeffs_709(16), c0 = coeffs_709(0);
@@ -81,6 +91,18 @@ static_assert(c0.y_r == 3484 && c0.y_g == 11717 && c0.y_b == 1183, "709/full Y r
 static_assert(c0.cb_r == -1877 && c0.cb_g == -6315 && c0.cb_b == 8192, "709/full Cb row");
 static_assert(c0.cr_r == 8191 && c0.cr_g == -7441 && c0.cr_b == -750, "709/full Cr row");
 static_assert(c0.y_scale == 16384 && c0.r_cr == 25800 && c0.g_cb == -3069 && c0.g_cr == -7671 && c0.b_cb == 30402, "709/full inverse");
+// BT.601, as the reference built with color-601 returns them for CS_DFL (tests/test_color601.py probes every depth)
+constexpr color_coeffs s8 = coeffs_601(8), s10 = coeffs_601(10), s16 = coeffs_601(16);
+static_assert(s8.y_r == 4207 && s8.y_g == 8260 && s8.y_b == 1604, "601/8 Y row");
+static_assert(s8.cb_r == -2428 && s8.cb_g == -4768 && s8.cb_b == 7196, "601/8 Cb row");
+static_assert(s8.cr_r == 7195 && s8.cr_g == -6026 && s8.cr_b == -1169, "601/8 Cr row");
+static_assert(s8.y_scale == 19077 && s8.r_cr == 26149 && s8.g_cb == -6419 && s8.g_cr == -13320 && s8.b_cb == 33050, "601/8 inverse");
+static_assert(s10.y_r == 4195 && s10.y_g == 8235 && s10.y_b == 1599 && s10.cb_r == -2421 && s10.cb_g == -4754 && s10.cb_b == 7175, "601/10 Y, Cb");
+static_assert(s10.cr_r == 7174 && s10.cr_g == -6008 && s10.cr_b == -1166, "601/10 Cr row");
+static_assert(s10.y_scale == 19133 && s10.r_cr == 26226 && s10.g_cb == -6438 && s10.g_cr == -13359 && s10.b_cb == 33148, "601/10 inverse");
+static_assert(s16.y_r == 4191 && s16.y_g == 8228 && s16.y_b == 1598 && s16.cb_r == -2419 && s16.cb_g == -4749 && s16.cb_b == 7168, "601/16 Y, Cb");
+static_assert(s16.cr_r == 7167 && s16.cr_g == -6002 && s16.cr_b == -1165, "601/16 Cr row");
+static_assert(s16.y_scale == 19152 && s16.r_cr == 26251 && s16.g_cb == -6444 && s16.g_cr == -13372 && s16.b_cb == 33179, "601/16 inverse");
 }  // namespace pin
 
 // ---- YCbCr -> YCbCr between two colour spaces (ugb200_jpeg_decode_to) ------------------------------------------------------------

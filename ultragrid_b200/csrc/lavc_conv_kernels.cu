@@ -244,13 +244,14 @@ struct rgb_src<SRC_RGB8> {
         }
 };
 
-/// DEPTH: output depth (coefficients of get_color_coeffs(CS_DFL, DEPTH)); SUB422: chroma of the even pixels only (r12l_to_yuv422pXXle, :776-787)
-template <int SRC, int DEPTH, bool SUB422>
+/// DEPTH: output depth (coefficients of get_color_coeffs(CS_DFL, DEPTH), from the set CS of color_space.h); SUB422: chroma of the even pixels only
+/// (r12l_to_yuv422pXXle, :776-787)
+template <int SRC, int DEPTH, bool SUB422, class CS = bt709>
 __global__ void __launch_bounds__(128) lavc_rgb_kernel(const uint8_t *__restrict__ in, long in_pitch, lavc_planes o, int width, int height, int groups,
                                                        bool vec, bool in_vec)
 {
         typedef rgb_src<SRC> S;
-        constexpr color_coeffs cf = coeffs_709(DEPTH);
+        constexpr color_coeffs cf = CS::at(DEPTH);
         constexpr int SHIFT = COMP_BASE + S::kDepth - DEPTH;
         const int gidx = blockIdx.x * blockDim.x + threadIdx.x;
         if (gidx >= groups) {
@@ -461,11 +462,11 @@ int ugb200_to_lavc_supported(int in, int f)
         }
 }
 
-int ugb200_to_lavc_convert(int in, int f, const struct ugb200_av_planes *out, const void *in_data, int width, int height, cuda_wrapper_stream_t stream)
+}  // extern "C"
+
+template <class CS>
+static int to_lavc_convert(int in, int f, const struct ugb200_av_planes *out, const void *in_data, int width, int height, cuda_wrapper_stream_t stream)
 {
-        if (!out || !in_data || width <= 0 || height <= 0 || !ugb200_to_lavc_supported(in, f)) {
-                return -1;
-        }
         cudaStream_t st = (cudaStream_t) stream;
         const lavc_fmt_info fi = fmt_info(f);
         lavc_planes o{};
@@ -532,7 +533,7 @@ int ugb200_to_lavc_convert(int in, int f, const struct ugb200_av_planes *out, co
         } else {
                 const int groups = (width + 7) / 8;
                 const dim3 grid((groups + 127) / 128, gy);
-#define UGB_RGB_LAUNCH(SRC, DEPTH, SUB) lavc_rgb_kernel<SRC, DEPTH, SUB><<<grid, 128, 0, st>>>(src, pitch, o, width, height, groups, vec, in_vec)
+#define UGB_RGB_LAUNCH(SRC, DEPTH, SUB) lavc_rgb_kernel<SRC, DEPTH, SUB, CS><<<grid, 128, 0, st>>>(src, pitch, o, width, height, groups, vec, in_vec)
 #define UGB_RGB_DEPTHS(SRC)                                                                       \
         switch (f) {                                                                              \
         case UGB_AV_YUV444P10LE: UGB_RGB_LAUNCH(SRC, 10, false); break;                           \
@@ -561,25 +562,46 @@ int ugb200_to_lavc_convert(int in, int f, const struct ugb200_av_planes *out, co
         return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }
 
+extern "C" {
+
+int ugb200_to_lavc_convert_cs(int in, int f, const struct ugb200_av_planes *out, const void *in_data, int width, int height, int cs,
+                              cuda_wrapper_stream_t stream)
+{
+        if (!out || !in_data || width <= 0 || height <= 0 || !ugb200_to_lavc_supported(in, f)) {
+                return -1;
+        }
+        switch (cs) {
+        case UGB_CS_DFL:
+        case UGB_CS_709: return to_lavc_convert<bt709>(in, f, out, in_data, width, height, stream);
+        case UGB_CS_601: return to_lavc_convert<bt601>(in, f, out, in_data, width, height, stream);
+        default: return -1;
+        }
+}
+
+int ugb200_to_lavc_convert(int in, int f, const struct ugb200_av_planes *out, const void *in_data, int width, int height, cuda_wrapper_stream_t stream)
+{
+        return ugb200_to_lavc_convert_cs(in, f, out, in_data, width, height, UGB_CS_709, stream);
+}
+
 // ---- hook shape: to_lavc_vid_conv_cuda_init / to_lavc_vid_conv_cuda / _destroy (to_lavc_vid_conv_cuda.h:60-65) -------------------------------
 struct ugb200_to_lavc_conv {
-        int in_codec, width, height, av_pixfmt;
+        int in_codec, width, height, av_pixfmt, cs;
         struct ugb200_av_planes planes;  // device memory, owned
         void *d_in;                      // staging of a host input frame
         size_t in_bytes;
         cudaStream_t stream;
 };
 
-struct ugb200_to_lavc_conv *ugb200_to_lavc_vid_conv_init(int in_codec, int width, int height, int av_pixfmt)
+struct ugb200_to_lavc_conv *ugb200_to_lavc_vid_conv_init_cs(int in_codec, int width, int height, int av_pixfmt, int cs)
 {
-        if (width <= 0 || height <= 0 || !ugb200_to_lavc_supported(in_codec, av_pixfmt)) {
+        if (width <= 0 || height <= 0 || !ugb200_to_lavc_supported(in_codec, av_pixfmt) || (cs != UGB_CS_DFL && cs != UGB_CS_601 && cs != UGB_CS_709)) {
                 return nullptr;
         }
         auto *s = new (std::nothrow) ugb200_to_lavc_conv();
         if (!s) {
                 return nullptr;
         }
-        s->in_codec = in_codec, s->width = width, s->height = height, s->av_pixfmt = av_pixfmt;
+        s->in_codec = in_codec, s->width = width, s->height = height, s->av_pixfmt = av_pixfmt, s->cs = cs;
         const lavc_fmt_info fi = fmt_info(av_pixfmt);
         bool ok = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking) == cudaSuccess;
         for (int i = 0; i < fi.planes && ok; ++i) {
@@ -601,6 +623,11 @@ struct ugb200_to_lavc_conv *ugb200_to_lavc_vid_conv_init(int in_codec, int width
         return s;
 }
 
+struct ugb200_to_lavc_conv *ugb200_to_lavc_vid_conv_init(int in_codec, int width, int height, int av_pixfmt)
+{
+        return ugb200_to_lavc_vid_conv_init_cs(in_codec, width, height, av_pixfmt, UGB_CS_709);
+}
+
 const struct ugb200_av_planes *ugb200_to_lavc_vid_conv(struct ugb200_to_lavc_conv *s, const char *in_data, int in_is_device)
 {
         if (!s || !in_data) {
@@ -613,7 +640,7 @@ const struct ugb200_av_planes *ugb200_to_lavc_vid_conv(struct ugb200_to_lavc_con
                 }
                 src = s->d_in;
         }
-        if (ugb200_to_lavc_convert(s->in_codec, s->av_pixfmt, &s->planes, src, s->width, s->height, s->stream) != 0 ||
+        if (ugb200_to_lavc_convert_cs(s->in_codec, s->av_pixfmt, &s->planes, src, s->width, s->height, s->cs, s->stream) != 0 ||
             cudaStreamSynchronize(s->stream) != cudaSuccess) {
                 return nullptr;
         }

@@ -23,7 +23,8 @@ __device__ __forceinline__ int clamp255(int v) { return min(max(v, 0), 255); }
 
 // ---- converters ----------------------------------------------------------------------------------
 // Each declares IN/OUT bytes per chunk, out_len(dst_len) = number of bytes the reference loop writes
-// for a given dst_len, and run().
+// for a given dst_len, and run().  A converter that reads colour coefficients takes their set as the template parameter CS
+// (bt709 / bt601, color_space.h); ugb200_pixfmt_convert_cs picks the instantiation.
 
 /// vc_copylinev210, pixfmt_conv.c:86-130: drop the 2 LSBs of each 10-bit sample; 16 B (6 px) -> 12 B
 struct conv_v210_uyvy {
@@ -197,6 +198,7 @@ struct conv_v210_y416 {
 
 /// vc_copylineV210toRGB, pixfmt_conv.c:2884-2940: top 8 bits of each sample, depth-8 coefficients, CLAMP_FULL (1..254);
 /// the loop runs while x < dst_len in steps of 18 bytes, i.e. it may write past dst_len up to the end of the last group
+template <class CS = bt709>
 struct conv_v210_rgb {  // fp32 like conv_yuv422_rgb: the sums stay below 2^24 (8-bit samples, depth-8 coefficients), >> 14 = round-down FMA
         static constexpr int IN = 128, OUT = 144;
         static __host__ int out_len(int dst_len) { return (dst_len + 17) / 18 * 18; }
@@ -208,7 +210,11 @@ struct conv_v210_rgb {  // fp32 like conv_yuv422_rgb: the sums stay below 2^24 (
         }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(8);
+                constexpr color_coeffs c = CS::at(8);
+                static_assert(239L * c.y_scale + 128L * c.b_cb < (1L << 24) && 239L * c.y_scale + 128L * c.r_cr < (1L << 24) &&
+                                      16L * c.y_scale + 128L * c.b_cb < (1L << 24) && 16L * c.y_scale + 128L * c.r_cr < (1L << 24) &&
+                                      239L * c.y_scale - 128L * (c.g_cb + c.g_cr) < (1L << 24),
+                              "fp32 must hold the sums exactly");
                 const float2 ys = make_float2((float) c.y_scale, (float) c.y_scale), ybias = make_float2(-8388624.0f, -8388624.0f),
                              cbias = make_float2(-8388736.0f, -8388736.0f);
 #pragma unroll
@@ -249,13 +255,14 @@ struct conv_v210_rgb {  // fp32 like conv_yuv422_rgb: the sums stay below 2^24 (
         }
 };
 /// vc_copylineV210toRG48, pixfmt_conv.c:2942-3002: all 10 bits, depth-10 coefficients, >> (COMP_BASE - 6), CLAMP_FULL at 16 bit
+template <class CS = bt709>
 struct conv_v210_rg48 {
         static constexpr int IN = 64, OUT = 144;
         static __host__ int out_len(int dst_len) { return (dst_len + 35) / 36 * 36; }
         static __device__ __forceinline__ uint32_t cf(int v) { return (uint32_t) min(max(v, 256), 65279); }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(10);
+                constexpr color_coeffs c = CS::at(10);
 #pragma unroll
                 for (int g = 0; g < 4; ++g) {
                         const uint32_t w0 = in[4 * g], w1 = in[4 * g + 1], w2 = in[4 * g + 2], w3 = in[4 * g + 3];
@@ -462,12 +469,13 @@ struct conv_444_uyvy {
 using conv_vuya_uyvy = conv_444_uyvy<4, 1, 2, 0, 7>;
 using conv_y416_uyvy = conv_444_uyvy<8, 1, 3, 5, 11>;
 /// vc_copylineVUYAtoRGB, :2705-2726 (depth-8 coefficients, CLAMP_FULL 1..254, runs while x < dst_len in steps of 3)
+template <class CS = bt709>
 struct conv_vuya_rgb {
         static constexpr int IN = 64, OUT = 48;
         static __host__ int out_len(int n) { return (n + 2) / 3 * 3; }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(8);
+                constexpr color_coeffs c = CS::at(8);
                 uint32_t o[48];
 #pragma unroll
                 for (int i = 0; i < 16; ++i) {
@@ -483,12 +491,13 @@ struct conv_vuya_rgb {
         }
 };
 /// vc_copylineRGBAtoVUYA, :2280-2302 (V U Y A; no clamp, bytes wrap)
+template <class CS = bt709>
 struct conv_rgba_vuya {
         static constexpr int IN = 16, OUT = 16;
         static __host__ int out_len(int n) { return n / 4 * 4; }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(8);
+                constexpr color_coeffs c = CS::at(8);
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                         const int r = in[i] & 0xff, g = (in[i] >> 8) & 0xff, b = (in[i] >> 16) & 0xff;
@@ -509,7 +518,7 @@ __device__ __forceinline__ int gh(const uint32_t *a)
 
 /// Y416 (U Y V A, 16 bit) -> RGB-like.  MODE 0: RG48 (vc_copylineY416toRG48, pixfmt_conv.c:2485-2514), 1: RGB (:1948-1976),
 /// 2: RGBA (:1978-2006), 3: R10k (:1917-1946).  int32 arithmetic wraps exactly like the reference's comp_type_t.
-template <int MODE>
+template <int MODE, class CS = bt709>
 struct conv_y416_rgbx {
         static constexpr int NPX = MODE == 0 ? 8 : MODE == 1 ? 16 : 4;
         static constexpr int IN = NPX * 8, OUT = NPX * (MODE == 0 ? 6 : MODE == 1 ? 3 : 4);
@@ -518,7 +527,7 @@ struct conv_y416_rgbx {
         static __device__ __forceinline__ void px(const uint32_t *in, uint32_t *o, const conv_params &p)
         {
                 if constexpr (K < NPX) {
-                        constexpr color_coeffs c = coeffs_709(16);
+                        constexpr color_coeffs c = CS::at(16);
                         constexpr int SH = COMP_BASE + (MODE == 0 ? 0 : MODE == 3 ? 6 : 8);
                         constexpr int LO = MODE == 0 ? 256 : MODE == 3 ? 4 : 1, HI = MODE == 0 ? 65279 : MODE == 3 ? 1019 : 254;  // CLAMP_FULL
                         const int u = gh<4 * K>(in) - 32768, y = c.y_scale * (gh<4 * K + 1>(in) - 4096), v = gh<4 * K + 2>(in) - 32768;
@@ -581,6 +590,7 @@ struct conv_y416_v210 {
 };
 
 /// RG48 -> Y416 (vc_copylineRG48toY416, :2451-2483) / Y216 (:2410-2449) with depth-16 coefficients; results stored as uint16 (wrap)
+template <class CS = bt709>
 struct conv_rg48_y416 {
         static constexpr int IN = 48, OUT = 64;
         static __host__ int out_len(int n) { return (n + 7) / 8 * 8; }
@@ -588,7 +598,7 @@ struct conv_rg48_y416 {
         static __device__ __forceinline__ void px(const uint32_t *in, uint32_t *out)
         {
                 if constexpr (K < 8) {
-                        constexpr color_coeffs c = coeffs_709(16);
+                        constexpr color_coeffs c = CS::at(16);
                         const int r = gh<3 * K>(in), g = gh<3 * K + 1>(in), b = gh<3 * K + 2>(in);
                         const uint32_t u = ((r * c.cb_r + g * c.cb_g + b * c.cb_b) >> COMP_BASE) + 32768, y = ((r * c.y_r + g * c.y_g + b * c.y_b) >> COMP_BASE) + 4096,
                                        v = ((r * c.cr_r + g * c.cr_g + b * c.cr_b) >> COMP_BASE) + 32768;
@@ -599,6 +609,7 @@ struct conv_rg48_y416 {
         }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &) { px<0>(in, out); }
 };
+template <class CS = bt709>
 struct conv_rg48_y216 {
         static constexpr int IN = 48, OUT = 32;
         static __host__ int out_len(int n) { return (n + 7) / 8 * 8; }
@@ -606,7 +617,7 @@ struct conv_rg48_y216 {
         static __device__ __forceinline__ void pair(const uint32_t *in, uint32_t *out)
         {
                 if constexpr (K < 4) {
-                        constexpr color_coeffs c = coeffs_709(16);
+                        constexpr color_coeffs c = CS::at(16);
                         const int r0 = gh<6 * K>(in), g0 = gh<6 * K + 1>(in), b0 = gh<6 * K + 2>(in), r1 = gh<6 * K + 3>(in), g1 = gh<6 * K + 4>(in),
                                   b1 = gh<6 * K + 5>(in);
                         const int y0 = ((r0 * c.y_r + g0 * c.y_g + b0 * c.y_b) >> COMP_BASE) + 4096, y1 = ((r1 * c.y_r + g1 * c.y_g + b1 * c.y_b) >> COMP_BASE) + 4096;
@@ -620,13 +631,14 @@ struct conv_rg48_y216 {
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &) { pair<0>(in, out); }
 };
 /// vc_copylineRG48toV210, :2354-2407: depth-10 coefficients, shift COMP_BASE + 6; chroma shifted per pixel, summed, C '/ 2'
+template <class CS = bt709>
 struct conv_rg48_v210 {
         static constexpr int IN = 144, OUT = 64;
         static __host__ int out_len(int n) { return n < 16 ? 0 : n / 16 * 16; }
         template <int P>  // pixel pair P of the chunk (12 pairs): y1, y2, u, v
         static __device__ __forceinline__ void fetch(const uint32_t *in, uint32_t &y1, uint32_t &y2, uint32_t &u, uint32_t &v)
         {
-                constexpr color_coeffs c = coeffs_709(10);
+                constexpr color_coeffs c = CS::at(10);
                 constexpr int OFF = COMP_BASE + 6;
                 const int r0 = gh<6 * P>(in), g0 = gh<6 * P + 1>(in), b0 = gh<6 * P + 2>(in), r1 = gh<6 * P + 3>(in), g1 = gh<6 * P + 4>(in), b1 = gh<6 * P + 5>(in);
                 y1 = (uint32_t) (((r0 * c.y_r + g0 * c.y_g + b0 * c.y_b) >> OFF) + 64);
@@ -652,12 +664,13 @@ struct conv_rg48_v210 {
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &) { group<0>(in, out); }
 };
 /// vc_copylineUYVYtoRG48, :1124-1130 = copylineYUVtoRGB with rgb16: each 8-bit result in the HIGH byte of a 16-bit sample
+template <class CS = bt709>
 struct conv_uyvy_rg48 {
         static constexpr int IN = 16, OUT = 48;
         static __host__ int out_len(int n) { return n < 12 ? 0 : n / 12 * 12; }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(8);
+                constexpr color_coeffs c = CS::at(8);
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                         const uint32_t w = in[i];
@@ -672,12 +685,13 @@ struct conv_uyvy_rg48 {
 };
 /// vc_copyliner10ktoY416, :294-329 (components widened to 16 bit, depth-16 coefficients) and vc_copylineR10ktoUYVY, :2318-2334
 /// (8-bit truncation, then the RGB -> UYVY body)
+template <class CS = bt709>
 struct conv_r10k_y416 {
         static constexpr int IN = 32, OUT = 64;
         static __host__ int out_len(int n) { return (n + 7) / 8 * 8; }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(16);
+                constexpr color_coeffs c = CS::at(16);
 #pragma unroll
                 for (int i = 0; i < 8; ++i) {
                         const int b1 = in[i] & 0xff, b2 = (in[i] >> 8) & 0xff, b3 = (in[i] >> 16) & 0xff, b4 = in[i] >> 24;
@@ -689,12 +703,13 @@ struct conv_r10k_y416 {
                 }
         }
 };
+template <class CS = bt709>
 struct conv_r10k_uyvy {
         static constexpr int IN = 32, OUT = 16;
         static __host__ int out_len(int n) { return (n + 3) / 4 * 4; }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(8);
+                constexpr color_coeffs c = CS::at(8);
 #pragma unroll
                 for (int i = 0; i < 4; ++i) {
                         int r[2], g[2], b[2];
@@ -714,12 +729,13 @@ struct conv_r10k_uyvy {
 
 /// R12L -> Y416 (vc_copylineR12LtoY416, :1478-1542; components << 4, depth-16 coefficients) and
 /// R12L -> UYVY (vc_copylineR12LtoUYVY, :1544-1638; depth-8 coefficients on 16-bit components, one shift of COMP_BASE + 8 (+1 for chroma))
+template <class CS = bt709>
 struct conv_r12l_y416 {
         static constexpr int IN = 144, OUT = 256;
         static __host__ int out_len(int n) { return (n + 63) / 64 * 64; }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(16);
+                constexpr color_coeffs c = CS::at(16);
 #pragma unroll
                 for (int g = 0; g < 4; ++g) {
 #pragma unroll
@@ -733,12 +749,13 @@ struct conv_r12l_y416 {
                 }
         }
 };
+template <class CS = bt709>
 struct conv_r12l_uyvy {
         static constexpr int IN = 144, OUT = 64;
         static __host__ int out_len(int n) { return (n + 15) / 16 * 16; }
         static __device__ __forceinline__ void run(const uint32_t *in, uint32_t *out, const conv_params &, const row_ctx &)
         {
-                constexpr color_coeffs c = coeffs_709(8);
+                constexpr color_coeffs c = CS::at(8);
 #pragma unroll
                 for (int g = 0; g < 4; ++g) {
 #pragma unroll
@@ -1016,28 +1033,35 @@ struct staged_default {
         struct staged_default<CONV> {                                                                                                         \
                 static constexpr int value = MODE;                                                                                            \
         };
-UGB_STAGED(conv_v210_rg48, 2)
+// converters that read colour coefficients: one form for every coefficient set (the sets differ in immediates only)
+#define UGB_STAGED_CS(MODE, ...)                                                                                                              \
+        template <class CS>                                                                                                                   \
+        struct staged_default<__VA_ARGS__> {                                                                                                  \
+                static constexpr int value = MODE;                                                                                            \
+        };
+UGB_STAGED_CS(2, conv_v210_rg48<CS>)
 UGB_STAGED(conv_r12l_rgbx<0>, 2)     // R12L -> RGB
 UGB_STAGED(conv_r12l_rgbx<1>, 2)     // R12L -> RGBA
 UGB_STAGED(conv_r12l_rgbx<2>, 2)     // R12L -> RG48
 UGB_STAGED(conv_r12l_rgbx<3>, 2)     // R12L -> R10k
-UGB_STAGED(conv_r12l_y416, 2)
+UGB_STAGED_CS(2, conv_r12l_y416<CS>)
 UGB_STAGED(conv_x_r12l<0>, 2)        // RGB  -> R12L
 UGB_STAGED(conv_x_r12l<1>, 2)        // RGBA -> R12L
 UGB_STAGED(conv_x_r12l<2>, 2)        // RG48 -> R12L
-UGB_STAGED(conv_x_r12l<3>, 2)        // Y416 -> R12L
+UGB_STAGED_CS(2, conv_x_r12l<3, CS>)  // Y416 -> R12L
 UGB_STAGED(conv_rgb_rgba, 2)
 UGB_STAGED(conv_bytemap<map_uyvy_y416>, 1)
-UGB_STAGED(conv_r10k_y416, 2)
+UGB_STAGED_CS(2, conv_r10k_y416<CS>)
 UGB_STAGED(conv_uyvy_v210, 2)
-UGB_STAGED(conv_vuya_rgb, 2)
-UGB_STAGED(conv_rg48_y416, 2)
+UGB_STAGED_CS(2, conv_vuya_rgb<CS>)
+UGB_STAGED_CS(2, conv_rg48_y416<CS>)
 UGB_STAGED(conv_r10k_rg48, 2)
 UGB_STAGED(conv_v210_y416, 2)
-UGB_STAGED(conv_rg48_v210, 2)
-UGB_STAGED(conv_rg48_y216, 3)
+UGB_STAGED_CS(2, conv_rg48_v210<CS>)
+UGB_STAGED_CS(3, conv_rg48_y216<CS>)
 UGB_STAGED(conv_v210_uyvy, 2)
 UGB_STAGED(conv_rg48_r10k, 2)
+#undef UGB_STAGED_CS
 #undef UGB_STAGED
 
 static int &staged_mode()
@@ -1098,16 +1122,22 @@ struct lean_default {
         struct lean_default<__VA_ARGS__> {                                                                                                    \
                 static constexpr bool value = true;                                                                                           \
         };
+#define UGB_LEAN_CS(...)                                                                                                                      \
+        template <class CS>                                                                                                                   \
+        struct lean_default<__VA_ARGS__> {                                                                                                    \
+                static constexpr bool value = true;                                                                                           \
+        };
 UGB_LEAN(conv_uyvy_rgba)
 UGB_LEAN(conv_r10k_rgba)
-UGB_LEAN(conv_uyvy_rg48)
-UGB_LEAN(conv_rgba_vuya)
-UGB_LEAN(conv_to_uyvy<2, 1, 0, 3>)     // BGR  -> UYVY
-UGB_LEAN(conv_to_uyvy<0, 1, 2, 4>)     // RGBA -> UYVY
+UGB_LEAN_CS(conv_uyvy_rg48<CS>)
+UGB_LEAN_CS(conv_rgba_vuya<CS>)
+UGB_LEAN_CS(conv_to_uyvy<2, 1, 0, 3, CS>)  // BGR  -> UYVY
+UGB_LEAN_CS(conv_to_uyvy<0, 1, 2, 4, CS>)  // RGBA -> UYVY
 UGB_LEAN(conv_rgba_r10k)
-UGB_LEAN(conv_y416_rgbx<3>)            // Y416 -> R10k
-UGB_LEAN(conv_y416_rgbx<2>)            // Y416 -> RGBA
+UGB_LEAN_CS(conv_y416_rgbx<3, CS>)         // Y416 -> R10k
+UGB_LEAN_CS(conv_y416_rgbx<2, CS>)         // Y416 -> RGBA
 UGB_LEAN(conv_vuya_uyvy)
+#undef UGB_LEAN_CS
 #undef UGB_LEAN
 
 template <class C>
@@ -1292,15 +1322,24 @@ extern "C" UGB_API int ugb200_pixfmt_supported(int in_codec, int out_codec)
         return 0;
 }
 
-extern "C" UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *dst, long dst_pitch, const void *src, long src_pitch,
-                                     int dst_len, int height, long src_size, int rshift, int gshift, int bshift,
-                                     cuda_wrapper_stream_t stream)
+/// the 8-bit limited-range YCbCr space of conv_yuv422_rgb for a coefficient set
+template <class CS>
+struct ycbcr8;
+template <>
+struct ycbcr8<bt709> {
+        using type = ycbcr_709;
+};
+template <>
+struct ycbcr8<bt601> {
+        using type = ycbcr_601;
+};
+
+/// ugb200_pixfmt_convert_cs with the coefficient set CS; converters that read no coefficients are the same instantiation for every CS
+template <class CS>
+static int pixfmt_convert(int in_codec, int out_codec, void *dst, long dst_pitch, const void *src, long src_pitch, int dst_len, int height, long src_size,
+                          int rshift, int gshift, int bshift, cudaStream_t s)
 {
-        cudaStream_t s = (cudaStream_t) stream;
         const conv_params p = { rshift, gshift, bshift, 0 };
-        if (dst == nullptr || src == nullptr || dst_len < 0 || height < 0) {
-                return -1;
-        }
         if (in_codec == out_codec && out_codec != UGB_RGBA && out_codec != UGB_RGB) {
                 return copy_rows(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, s);  // vc_memcpy (pixfmt_conv.c:2529-2536)
         }
@@ -1312,19 +1351,19 @@ extern "C" UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *
         case UGB_UYVY * 256 + UGB_YUYV:
                 return launch_line<conv_yuyv_uyvy>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_UYVY * 256 + UGB_RGB:
-                return launch_line<conv_yuv422_rgb<1, 3, 0, 2>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
+                return launch_line<conv_yuv422_rgb<1, 3, 0, 2, typename ycbcr8<CS>::type>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_YUYV * 256 + UGB_RGB:
-                return launch_line<conv_yuv422_rgb<0, 2, 1, 3>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
+                return launch_line<conv_yuv422_rgb<0, 2, 1, 3, typename ycbcr8<CS>::type>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_UYVY * 256 + UGB_RGBA:
                 return launch_line<conv_uyvy_rgba>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_RGB * 256 + UGB_UYVY:
-                return launch_line<conv_to_uyvy<0, 1, 2, 3>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
+                return launch_line<conv_to_uyvy<0, 1, 2, 3, CS>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_BGR * 256 + UGB_UYVY:
-                return launch_line<conv_to_uyvy<2, 1, 0, 3>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
+                return launch_line<conv_to_uyvy<2, 1, 0, 3, CS>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_RGBA * 256 + UGB_UYVY:
-                return launch_line<conv_to_uyvy<0, 1, 2, 4>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
+                return launch_line<conv_to_uyvy<0, 1, 2, 4, CS>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_RG48 * 256 + UGB_UYVY:
-                return launch_line<conv_to_uyvy<1, 3, 5, 6>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
+                return launch_line<conv_to_uyvy<1, 3, 5, 6, CS>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_RGB * 256 + UGB_RGBA:
                 return launch_line<conv_rgb_rgba>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_RGBA * 256 + UGB_RGB:
@@ -1348,10 +1387,10 @@ extern "C" UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *
         case UGB_v210 * 256 + UGB_Y416:
                 return launch_line<conv_v210_y416>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
         case UGB_v210 * 256 + UGB_RGB:
-                return launch_line<conv_v210_rgb>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
-#define UGB_CASE(IN_C, OUT_C, CONV)                                                                                                         \
+                return launch_line<conv_v210_rgb<CS>>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
+#define UGB_CASE(IN_C, OUT_C, ...)                                                                                                          \
         case IN_C * 256 + OUT_C:                                                                                                            \
-                return launch_line<CONV>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
+                return launch_line<__VA_ARGS__>(dst, dst_pitch, src, src_pitch, dst_len, height, src_size, p, s);
                 UGB_CASE(UGB_RG48, UGB_RGB, conv_bytemap<map_rg48_rgb>)
                 UGB_CASE(UGB_RGBA, UGB_RG48, conv_bytemap<map_rgba_rg48>)
                 UGB_CASE(UGB_RGB, UGB_RG48, conv_bytemap<map_rgb_rg48>)
@@ -1367,32 +1406,32 @@ extern "C" UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *
                 UGB_CASE(UGB_RG48, UGB_RGBA, conv_rg48_rgba)
                 UGB_CASE(UGB_VUYA, UGB_UYVY, conv_vuya_uyvy)
                 UGB_CASE(UGB_Y416, UGB_UYVY, conv_y416_uyvy)
-                UGB_CASE(UGB_VUYA, UGB_RGB, conv_vuya_rgb)
-                UGB_CASE(UGB_RGBA, UGB_VUYA, conv_rgba_vuya)
-                UGB_CASE(UGB_Y416, UGB_RG48, conv_y416_rgbx<0>)
-                UGB_CASE(UGB_Y416, UGB_RGB, conv_y416_rgbx<1>)
-                UGB_CASE(UGB_Y416, UGB_RGBA, conv_y416_rgbx<2>)
-                UGB_CASE(UGB_Y416, UGB_R10k, conv_y416_rgbx<3>)
+                UGB_CASE(UGB_VUYA, UGB_RGB, conv_vuya_rgb<CS>)
+                UGB_CASE(UGB_RGBA, UGB_VUYA, conv_rgba_vuya<CS>)
+                UGB_CASE(UGB_Y416, UGB_RG48, conv_y416_rgbx<0, CS>)
+                UGB_CASE(UGB_Y416, UGB_RGB, conv_y416_rgbx<1, CS>)
+                UGB_CASE(UGB_Y416, UGB_RGBA, conv_y416_rgbx<2, CS>)
+                UGB_CASE(UGB_Y416, UGB_R10k, conv_y416_rgbx<3, CS>)
                 UGB_CASE(UGB_Y416, UGB_v210, conv_y416_v210)
-                UGB_CASE(UGB_RG48, UGB_Y416, conv_rg48_y416)
-                UGB_CASE(UGB_RG48, UGB_Y216, conv_rg48_y216)
-                UGB_CASE(UGB_RG48, UGB_v210, conv_rg48_v210)
-                UGB_CASE(UGB_UYVY, UGB_RG48, conv_uyvy_rg48)
-                UGB_CASE(UGB_R10k, UGB_Y416, conv_r10k_y416)
-                UGB_CASE(UGB_R10k, UGB_UYVY, conv_r10k_uyvy)
-                UGB_CASE(UGB_v210, UGB_RG48, conv_v210_rg48)
+                UGB_CASE(UGB_RG48, UGB_Y416, conv_rg48_y416<CS>)
+                UGB_CASE(UGB_RG48, UGB_Y216, conv_rg48_y216<CS>)
+                UGB_CASE(UGB_RG48, UGB_v210, conv_rg48_v210<CS>)
+                UGB_CASE(UGB_UYVY, UGB_RG48, conv_uyvy_rg48<CS>)
+                UGB_CASE(UGB_R10k, UGB_Y416, conv_r10k_y416<CS>)
+                UGB_CASE(UGB_R10k, UGB_UYVY, conv_r10k_uyvy<CS>)
+                UGB_CASE(UGB_v210, UGB_RG48, conv_v210_rg48<CS>)
                 UGB_CASE(UGB_DVS10, UGB_UYVY, conv_bytemap<map_dvs10_uyvy>)
                 UGB_CASE(UGB_DVS10, UGB_v210, conv_dvs10_v210)
                 UGB_CASE(UGB_R12L, UGB_RGB, conv_r12l_rgbx<0>)
                 UGB_CASE(UGB_R12L, UGB_RGBA, conv_r12l_rgbx<1>)
                 UGB_CASE(UGB_R12L, UGB_RG48, conv_r12l_rgbx<2>)
                 UGB_CASE(UGB_R12L, UGB_R10k, conv_r12l_rgbx<3>)
-                UGB_CASE(UGB_R12L, UGB_Y416, conv_r12l_y416)
-                UGB_CASE(UGB_R12L, UGB_UYVY, conv_r12l_uyvy)
+                UGB_CASE(UGB_R12L, UGB_Y416, conv_r12l_y416<CS>)
+                UGB_CASE(UGB_R12L, UGB_UYVY, conv_r12l_uyvy<CS>)
                 UGB_CASE(UGB_RGB, UGB_R12L, conv_x_r12l<0>)
                 UGB_CASE(UGB_RGBA, UGB_R12L, conv_x_r12l<1>)
                 UGB_CASE(UGB_RG48, UGB_R12L, conv_x_r12l<2>)
-                UGB_CASE(UGB_Y416, UGB_R12L, conv_x_r12l<3>)
+                UGB_CASE(UGB_Y416, UGB_R12L, conv_x_r12l<3, CS>)
 #undef UGB_CASE
         case UGB_BGR * 256 + UGB_RGB: {
                 const conv_params q = { 16, 8, 0, 0 };  // vc_copylineBGRtoRGB
@@ -1400,6 +1439,33 @@ extern "C" UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *
         }
         }
         return -4;  // no decoder (get_decoder_from_to() == NULL, pixfmt_conv.c:3122-3124)
+}
+
+extern "C" UGB_API int ugb200_pixfmt_convert_cs(int in_codec, int out_codec, void *dst, long dst_pitch, const void *src, long src_pitch, int dst_len,
+                                                int height, long src_size, int rshift, int gshift, int bshift, int cs, cuda_wrapper_stream_t stream)
+{
+        if (dst == nullptr || src == nullptr || dst_len < 0 || height < 0) {
+                return -1;
+        }
+        switch (cs) {
+        case UGB_CS_DFL:
+        case UGB_CS_709:
+                return pixfmt_convert<bt709>(in_codec, out_codec, dst, dst_pitch, src, src_pitch, dst_len, height, src_size, rshift, gshift, bshift,
+                                             (cudaStream_t) stream);
+        case UGB_CS_601:
+                return pixfmt_convert<bt601>(in_codec, out_codec, dst, dst_pitch, src, src_pitch, dst_len, height, src_size, rshift, gshift, bshift,
+                                             (cudaStream_t) stream);
+        default:
+                return -1;
+        }
+}
+
+extern "C" UGB_API int ugb200_pixfmt_convert(int in_codec, int out_codec, void *dst, long dst_pitch, const void *src, long src_pitch,
+                                     int dst_len, int height, long src_size, int rshift, int gshift, int bshift,
+                                     cuda_wrapper_stream_t stream)
+{
+        return ugb200_pixfmt_convert_cs(in_codec, out_codec, dst, dst_pitch, src, src_pitch, dst_len, height, src_size, rshift, gshift, bshift, UGB_CS_709,
+                                        stream);
 }
 
 // ---- src/cuda_wrapper/kernels.cu under its own names (include/cuda_wrapper_kernels.hpp) ------------------------------------------------

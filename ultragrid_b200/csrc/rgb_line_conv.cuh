@@ -170,8 +170,8 @@ struct conv_r12l_rgbx {
 };
 
 /// X -> R12L.  SRC 0: RGB, 1: RGBA (vc_copylineRGB_AtoR12L, :1258-1334: 8-bit << 4), 2: RG48 (vc_copylineRG48toR12L, :1701-1826: 16-bit >> 4),
-/// 3: Y416 (vc_copylineY416toR12L, :1828-1915: depth-16 coefficients, >> COMP_BASE + 4, CLAMP_FULL 12 bit)
-template <int SRC>
+/// 3: Y416 (vc_copylineY416toR12L, :1828-1915: depth-16 coefficients of CS, >> COMP_BASE + 4, CLAMP_FULL 12 bit)
+template <int SRC, class CS = bt709>
 struct conv_x_r12l {
         static constexpr int IN = SRC == 0 ? 96 : SRC == 1 ? 128 : SRC == 2 ? 192 : 256, OUT = 144;
         static __host__ int out_len(int n) { return SRC == 3 ? (n + 35) / 36 * 36 : n / 36 * 36; }
@@ -193,7 +193,7 @@ struct conv_x_r12l {
                                 r = ((in[o >> 1] >> (16 * (o & 1))) & 0xffff) >> 4, g = ((in[(o + 1) >> 1] >> (16 * ((o + 1) & 1))) & 0xffff) >> 4,
                                 b = ((in[(o + 2) >> 1] >> (16 * ((o + 2) & 1))) & 0xffff) >> 4;
                         } else {
-                                constexpr color_coeffs c = coeffs_709(16);
+                                constexpr color_coeffs c = CS::at(16);
                                 const int u = (int) (in[2 * px] & 0xffff) - 32768, y = c.y_scale * ((int) (in[2 * px] >> 16) - 4096), v = (int) (in[2 * px + 1] & 0xffff) - 32768;
                                 r = clampr((y + v * c.r_cr) >> (COMP_BASE + 4), 16, 4079), g = clampr((y + u * c.g_cb + v * c.g_cr) >> (COMP_BASE + 4), 16, 4079),
                                 b = clampr((y + u * c.b_cb) >> (COMP_BASE + 4), 16, 4079);

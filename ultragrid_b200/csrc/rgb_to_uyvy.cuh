@@ -22,8 +22,8 @@ __device__ __forceinline__ uint32_t pack4(uint32_t b0, uint32_t b1, uint32_t b2,
 
 /// vc_copylineToUYVY, pixfmt_conv.c:1008-1053: RGB-like (ROFF/GOFF/BOFF within PIX bytes) -> UYVY.
 /// y = (RGB_TO_Y >> 14) + 16 unclamped; chroma = ((cb0 + cb1) / 2 >> 14) + 128 with C '/' truncation;
-/// bytes stored & 0xFF.  Used by RGB (:2061), BGR (:2271), RGBA (:2316), RG48 (:2343, high bytes).
-template <int ROFF, int GOFF, int BOFF, int PIX>
+/// bytes stored & 0xFF.  Used by RGB (:2061), BGR (:2271), RGBA (:2316), RG48 (:2343, high bytes).  CS: coefficient set (color_space.h).
+template <int ROFF, int GOFF, int BOFF, int PIX, class CS = bt709>
 struct conv_to_uyvy {
         static constexpr int NPX = 16 / (PIX == 3 ? 1 : PIX == 4 ? 2 : 2);  // 16, 8 (RGBA), 8 (RG48)
         static constexpr int IN = NPX * PIX, OUT = NPX * 2;
@@ -31,7 +31,7 @@ struct conv_to_uyvy {
         template <int K>
         static __device__ __forceinline__ void pair(const uint32_t *in, uint32_t *out)
         {
-                constexpr color_coeffs c = coeffs_709(8);
+                constexpr color_coeffs c = CS::at(8);
                 constexpr int P0 = 2 * K * PIX, P1 = P0 + PIX;
                 const int r0 = gb<P0 + ROFF>(in), g0 = gb<P0 + GOFF>(in), b0 = gb<P0 + BOFF>(in);
                 const int r1 = gb<P1 + ROFF>(in), g1 = gb<P1 + GOFF>(in), b1 = gb<P1 + BOFF>(in);
